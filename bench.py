@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- train-step/s (and Mrays/s) of the GS-SDF hot path on B200 (BASELINE.json metric).
+"""bench.py -- train-step/s (and Mrays/s) of the GS-SDF hot path on H100 (BASELINE.json metric).
 
 A "step" is one pass of the hot path (SURVEY.md section 3.2 [A]-[D], rows a1-a12 + f-1 + the optimiser half of f-3 of section 8) over one
 camera per rank: SDF stage on 32768 ray samples (hash grid + MLP, BCE + analytic eikonal + align with the tcnn double backward) ->
@@ -13,7 +13,7 @@ gradient is all-reduced over NCCL every step in two overlapped segments and ever
   e2e   : the same through the public API with HOST buffers: per step the camera (viewmat, K) and the
           ground-truth image are copied from pinned host memory and the loss is read back (D2H)
   roofline     : dominant kernel (raster backward): algorithmic bytes (SURVEY 8d) on the intersections the launch PROCESSES / CUDA-event
-                 time, plus the issue-slot fraction (the bound that actually applies) when an ncu instruction count is committed
+                 time
   stock_cuda   : the reference fork's own CUDA kernels (oracle/_ref/gsplat_ref.so, compiled from /root/reference, test infrastructure) on
                  the same tensors on the same GPU, per stage, beside ours (SURVEY 8d / BASELINE.md 3.1-2) -- never part of the product path
   cpu_baseline : config c1 (256x256, 50 k splats, SH 0, MLP 2x32) run FOR REAL on the CPU oracle port incl. Adam (median step, SURVEY 8d),
@@ -59,7 +59,7 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -122,19 +122,6 @@ def pci_bus_id():
         return f"{p.pci_domain_id:08x}:{p.pci_bus_id:02x}:{p.pci_device_id:02x}.0"
     except Exception:
         return None
-
-
-def ncu_profile(kernel):
-    """Per-launch figures of `kernel` from the committed ncu --set full capture of this round (profiles/r2_traffic.json, else round 1's):
-    {dram_bytes_per_launch, inst_executed_per_launch, source}; empty when nothing is committed."""
-    for name in ("r2_traffic.json", "r1_traffic.json"):
-        try:
-            d = json.load(open(os.path.join(ROOT, "profiles", name))).get(kernel)
-            if d:
-                return dict(d, source="profiles/" + name)
-        except Exception:
-            pass
-    return {}
 
 
 def cpu_dssim(x, y, w):
@@ -389,13 +376,16 @@ def main():
                     "even while a dense all-reduce is in flight")
     ap.add_argument("--dense-allreduce", action="store_true", help="A/B (N > 1): always all-reduce the dense splat segment (no sparse row exchange)")
     ap.add_argument("--nccl-high-priority", action="store_true", help="A/B (N > 1): run NCCL's kernels on a high-priority stream")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed (losses, "
+                    "rendered image and normals, updated parameters) as DIR/<name>.npy; arrays too large for the 64 MB total are fixed, "
+                    "seeded samples of their elements")
     ap.add_argument("--l2-persist", action="store_true", help="A/B: pin the fp16 hash-table shadow in L2 (gssdf_l2_persist); measured: no effect")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     W, H, N, deg, isect_cap = WORKLOADS[args.workload]
     cfg = {"workload": f"{args.workload}: {W}x{H}, {N} splats, SH deg {deg}, synthetic box scene seed 0 (SURVEY 8d), tile 16, packed, "
-                       f"1 camera/rank/step", "timing": "CUDA events; inputs (232 B/splat state + images) exceed the 126 MB L2, no flush",
+                       f"1 camera/rank/step", "timing": "CUDA events; inputs (232 B/splat state + images) exceed the 50 MB L2, no flush",
            "parallelism": (f"image-parallel dp{world}, replicated state, one pool of 8 camera poses, rank r renders pose (step + r * {max(8 // world, 1)}) mod 8"
                            f"{' (--same-cameras: the same pose on every rank)' if args.same_cameras else ''}, 2 NCCL exchanges/step: SDF segment (all-reduce) under "
                            f"the render backward; splat segment after the backward, as an all-gather of the ranks' visible rows when they are "
@@ -553,10 +543,10 @@ def main():
         randn_buf.normal_()  # the reference draws randns on the device every render (Projection.cpp:728)
         with T.sdf_stage():
             ray_xyz, ray_gt, ray_cnt = SP.draw(i)
-        loss, _sdf_loss = DP.step(V, Kc, gts[cam_of(i)], ray_xyz, ray_gt, randn_buf, ray_n_live=ray_cnt)
+        loss, sdf_loss = DP.step(V, Kc, gts[cam_of(i)], ray_xyz, ray_gt, randn_buf, ray_n_live=ray_cnt)
         DEN.update_state()  # NeuralGS::update_state: per-iteration densification statistics (the every-100-iterations surgery is not timed)
         R._mark("densify_stats")
-        return loss
+        return loss, sdf_loss
 
     # end-to-end path: every step's inputs (camera pose, intrinsics, ground-truth image) come from pinned HOST memory and the loss is
     # read back to the host every step. The copy of step i+1's inputs is enqueued on a copy stream while step i computes (two device
@@ -631,11 +621,15 @@ def main():
     torch.cuda.synchronize()
     sampler = ClockSampler(local, pci_bus_id()) if rank == 0 else None
 
+    last_out = {}
+
     def step_prof(i):
         R.prof_fwd, R.prof_bwd = prof_f[i], prof_b[i]
-        step_resident(i)
+        last_out["loss"], last_out["sdf_loss"] = step_resident(i)
 
     ms_total = timed(step_prof, args.steps, sampler)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(last_out, render_colors=R.out_colors, render_normals=R.out_normals, params=T.params))
     fwd_ms = [a.elapsed_time(b) for a, b in prof_f]
     bwd_ms = [a.elapsed_time(b) for a, b in prof_b]
     R.prof_fwd = R.prof_bwd = None
@@ -692,15 +686,6 @@ def main():
         t_bwd = float(np.mean(bwd_ms)) * 1e-3
         t_fwd = float(np.mean(fwd_ms)) * 1e-3
         achieved = alg_bwd / t_bwd / 1e9
-        prof = ncu_profile("raster2dgs_bwd_kernel")
-        issue = None
-        if prof.get("inst_executed_per_launch") and clocks and clocks.get("sm_mhz"):
-            sms = torch.cuda.get_device_properties(dev).multi_processor_count
-            slots_avail = sms * 4 * clocks["sm_mhz"] * 1e6 * t_bwd  # one warp instruction per SM sub-partition per clock
-            issue = {"inst_executed_per_launch": prof["inst_executed_per_launch"], "issue_slots_available": slots_avail,
-                     "frac": prof["inst_executed_per_launch"] / slots_avail, "source": prof.get("source"),
-                     "note": "warp instructions (ncu smsp__inst_executed.sum of the committed capture) / (SMs x 4 x measured SM clock x "
-                             "event time): the bound this kernel actually runs against"}
         line = {"metric": "train_steps_per_s", "value": value, "unit": "step/s", "n_gpus": world, "steps": args.steps,
                 "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "f32", "data": "synthetic", "config": cfg, "mrays_per_s": value * P / 1e6, "clocks": clocks,
@@ -715,22 +700,22 @@ def main():
                                  "isotropic -> backward, Adam over all parameter groups, densification statistics (update_state); not in the "
                                  "step: the every-100-iterations grow / split / prune surgery of NeuralGS::train_callback",
                 "roofline": {"kernel": "raster2dgs_bwd_kernel", "bound": "hbm", "achieved": achieved, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                             "frac": achieved / pk["hbm_gbs"], "traffic": prof.get("dram_bytes_per_launch"), "peak_source": pk_kind,
+                             "frac": achieved / pk["hbm_gbs"], "peak_source": pk_kind,
                              "algorithmic_bytes": alg_bwd, "kernel_ms": t_bwd * 1e3,
                              "units": {"I_processed": I_kept, "I_reference_aabb": I, "P": P, "nnz": nnz},
                              "frac_on_reference_units": alg_bwd_ref / t_bwd / 1e9 / pk["hbm_gbs"],
-                             "issue_slots": issue,
                              "note": "frac = SURVEY 8d bytes on the intersections the launch processes (after exact pre-sort culling) / event "
-                                     "time / measured copy bandwidth. The kernel is instruction-issue bound, not HBM bound (measured DRAM "
-                                     "traffic is below the algorithmic bytes): see issue_slots and profiles/",
+                                     "time / peak HBM bandwidth (peak_source)",
                              "raster_fwd": {"achieved": alg_fwd / t_fwd / 1e9, "frac": alg_fwd / t_fwd / 1e9 / pk["hbm_gbs"],
                                             "kernel_ms": t_fwd * 1e3, "algorithmic_bytes": alg_fwd}},
                 "splat_exchange_steps": {"visible_rows": DP.sparse_steps, "dense_allreduce": DP.dense_steps} if world > 1 else None,
                 "counts": cnt, "counts_end": cnt_end, "sdf_counts": sdf_counts, "loss_end": last_loss, "loss_finite": bool(np.isfinite(last_loss)),
-                "stage_ms": stage_ms}
+                "stage_ms": stage_ms,
+                # every device buffer of the library is a torch tensor, so the allocator's peak is the workload's footprint
+                "device_memory_peak_gib": torch.cuda.max_memory_allocated(dev) / 2 ** 30}
         if world == 1 and not args.no_stock_cuda:
             try:
-                line["stock_cuda"] = run_stock_cuda(torch, S, sc_act, cams, gts, W, H, deg, dev, stage_ms)
+                line["stock_cuda"] = run_stock_cuda(torch, S, sc_act, cams, gts, W, H, deg, dev, stage_ms, steps=args.steps)
             except Exception as e:  # test infrastructure missing on this box: say so, never fail the bench
                 line["stock_cuda"] = {"unavailable": f"{type(e).__name__}: {e}"[:300]}
         if world == 1 and not args.no_cpu_baseline:
@@ -756,12 +741,12 @@ def main():
                 torch.cuda.synchronize()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
-                for i in range(50):
+                for i in range(args.steps):
                     c1_step(i)
                 e1.record()
                 torch.cuda.synchronize()
-                gpu_c1 = 50e3 / e0.elapsed_time(e1)
-                cb["gpu_same_config"] = {"value": gpu_c1, "unit": "step/s", "ms_per_step": 1e3 / gpu_c1, "steps": 50,
+                gpu_c1 = args.steps * 1e3 / e0.elapsed_time(e1)
+                cb["gpu_same_config"] = {"value": gpu_c1, "unit": "step/s", "ms_per_step": 1e3 / gpu_c1, "steps": args.steps,
                                          "counts": T1.R.read_counts(), "ratio_gpu_over_cpu": gpu_c1 / cb["value"]}
             except Exception as e:
                 cb["gpu_same_config"] = {"unavailable": f"{type(e).__name__}: {e}"[:300]}
@@ -770,6 +755,19 @@ def main():
     if world > 1:
         dist.destroy_process_group()
     return 0
+
+
+def dump_outputs(out_dir, arrays, budget=60 << 20):
+    """Writes each array as out_dir/<name>.npy in float32. An array larger than its equal share of `budget` bytes is replaced by the
+    elements at a fixed, seeded set of flat indices (sorted; the same set for the same array size), so that two builds run with the same
+    arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = budget // 4 // len(arrays)
+    for name, a in arrays.items():
+        a = a.detach().float().cpu().numpy()
+        if a.size > share:
+            a = a.reshape(-1)[np.sort(np.random.default_rng(0).choice(a.size, share, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def run_stock_cuda(torch, S, sc_act, cams, gts, W, H, deg, dev, ours_stage_ms, steps=5):
@@ -835,7 +833,7 @@ def run_stock_cuda(torch, S, sc_act, cams, gts, W, H, deg, dev, ours_stage_ms, s
         info = {"nnz": int(gid.shape[0]), "n_isects": int(flatten_ids.shape[0])}
     st = {k: float(np.median(v)) for k, v in acc.items()}  # median: a stray cudaMalloc in one run must not colour the stage table
     total = float(sum(st.values()))
-    out = {"kind": "reference fork CUDA kernels (gsplat 2DGS path of GS-SDF) compiled for sm_100a with the reference's flags (-O3 "
+    out = {"kind": "reference fork CUDA kernels (gsplat 2DGS path of GS-SDF) compiled for sm_90a with the reference's flags (-O3 "
                    "--use_fast_math), same GPU, same tensors", "stage_ms": st, "splat_chain_ms": total, "steps": steps, "counts": info,
            "covers": "splat chain only (a2-a7): no losses, no SDF stages, no optimiser"}
     if ours_stage_ms:

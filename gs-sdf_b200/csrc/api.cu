@@ -14,7 +14,7 @@ void set_error(const char *fmt, ...) {
 }  // namespace gssdf
 
 extern "C" const char *gssdf_last_error(void) { return gssdf::g_err; }
-extern "C" const char *gssdf_version(void) { return "gssdf_b200 0.1 sm_100a"; }
+extern "C" const char *gssdf_version(void) { return "gssdf_b200 0.1 sm_90a"; }
 extern "C" int32_t gssdf_abi_revision(void) { return GSSDF_ABI_REVISION; }
 
 extern "C" int gssdf_l2_persist(const void *ptr, size_t bytes, float hit_ratio, gssdf_stream_t stream) {

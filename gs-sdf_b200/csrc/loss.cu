@@ -7,7 +7,7 @@
 // (loss_utils.cpp:6-14), an asymmetric 11-tap profile, reproduced here bit-for-bit in intent (the backward therefore uses the
 // flipped taps).
 //
-// B200 design: two streaming kernels instead of ~40 ATen launches. A WARP owns a strip of 32 image columns of one colour channel and
+// Design: two streaming kernels instead of ~40 ATen launches. A WARP owns a strip of 32 image columns of one colour channel and
 // marches down a band of rows: per input row it stages the 42 strip + halo values of x and y in a private shared-memory row (the only
 // shared memory used; no CTA-wide barrier anywhere), every lane runs the horizontal 11-tap pass of the five products for its column
 // (22 conflict-free shared loads), and the vertical pass lives in REGISTERS as a ring of 11 x 5 partial sums -- one input row updates the
@@ -215,10 +215,10 @@ extern "C" size_t gssdf_dssim_workspace_bytes(int32_t C, int32_t W, int32_t H) {
 }
 
 // rows per band: a warp marches (band + 10) row steps and the launch takes ceil(CTAs / resident CTAs) rounds of them (the kernels
-// run at the latency of a row step, not at an SM throughput limit: ncu, profiles/): a taller band amortises the 10 halo rows, a
+// run at the latency of a row step, not at an SM throughput limit): a taller band amortises the 10 halo rows, a
 // partial last round wastes most of a round. Ties go to the shorter band.
 static int ssim_band_height(const void *kernel, int W, int H, int C) {
-    int dev = 0, sms = 148, per_sm = 4;
+    int dev = 0, sms = 132, per_sm = 4;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kSsimWarps * 32, 0) != cudaSuccess || per_sm < 1) per_sm = 4;

@@ -9,7 +9,7 @@
 // The reference traces breadth-first: per octree level one decide kernel over all (ray, node) proposals, a CUB scan, a blocking
 // device->host copy of the proposal count, an at::empty and a subdivide kernel -- ~5 launches + 1 host sync per level (9 levels for a
 // 14 m map at 5 cm leaves), followed by ~25 ATen kernels with nonzero()/index_select host syncs for the sample assembly.
-// B200 design: each ray walks the octree DEPTH-first with a register stack, expanding children in the reference's front-to-back
+// Design: each ray walks the octree DEPTH-first with a register stack, expanding children in the reference's front-to-back
 // VOXEL_ORDER, which reproduces the reference's nugget sequence exactly (ray-major; a breadth-first expansion that keeps proposals in
 // place is the depth-first leaf order). Two traversals (count, write) around one scan give packed outputs without any host sync; the
 // sample assembly is one candidate kernel + one scan + one stable compaction. The octree (a few hundred KB) is L1/L2 resident.

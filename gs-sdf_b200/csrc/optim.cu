@@ -200,7 +200,7 @@ static int rows_launch(const gssdf_rows_args *a, gssdf_stream_t stream, bool pac
     }
     for (int i = a->n_segments; i <= GSSDF_ROWS_MAX_SEGMENTS; ++i) plan.start[i] = c;
     plan.stride = c;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int64_t want = cdiv(a->cap_rows * (int64_t)c, (int64_t)256);

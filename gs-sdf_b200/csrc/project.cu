@@ -3,7 +3,7 @@
 // Behaviour follows gsplat::projection_2dgs_packed_fwd/_bwd of the reference fork
 // (GSF/csrc/Projection.cpp:654-865, kernels GSF/csrc/Projection2DGSPacked.cu:18-217,298-501,
 // VJP GSF/csrc/Projection2DGS.cuh:10-90, quaternion helpers GSF/include/Utils.cuh:142-189).
-// Design differences (B200-first):
+// Design differences:
 //   * no host sync: count -> single-CTA scan -> compact write, nnz stays on the device;
 //   * splat attributes are staged through shared memory with 128-bit loads;
 //   * randns is an input (the reference draws it on the host after its sync);

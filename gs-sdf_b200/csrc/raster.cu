@@ -7,7 +7,7 @@
 //   depth = u*M_w.x + v*M_w.y + M_w.z ; alpha = min(0.999, o*exp(-(u^2+v^2)/2))
 //   skip if zeta.z == 0, depth < 0.05, alpha < 1/255 ; stop when T*(1-alpha) <= 1e-4
 //
-// B200-first design
+// Design
 //   * one 64-byte render record per visible splat (M[9], opacity, rgb[3], normal[3]) packed once per
 //     call; a tile's CTA gathers the records of its depth-sorted list with per-record TMA bulk copies
 //     (cp.async.bulk, mbarrier complete_tx) into a 2-stage shared-memory ring, so the per-pixel loop

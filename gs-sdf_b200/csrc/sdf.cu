@@ -8,15 +8,15 @@
 //   hash / index / scale helpers      TCNN/include/tiny-cuda-nn/common_device.h:631-655,690-718,842-855
 //   decoder torch::nn::Sequential     local_map.cpp:29-42 (Linear+ReLU x (1+geo_num_layer), Linear -> 2)
 //
-// B200-first design: ONE kernel per direction. A CTA owns a tile of points; the 32 encoded features and
+// Design: ONE kernel per direction. A CTA owns a tile of points; the 32 encoded features and
 // every 64-wide hidden activation live in shared memory only (the reference writes/reads [n,32] half +
 // [n,64] fp32 per layer through HBM and launches >= 12 kernels per get_sdf). The fp16 table (30.5 MB) is
-// L2-resident on B200 (126 MB L2); the fp32 master is cast to its fp16 shadow once per optimiser step, not on
+// L2-resident on H100 (50 MB L2); the fp32 master is cast to its fp16 shadow once per optimiser step, not on
 // every forward. The backward kernel is persistent (grid = k x SMs): decoder weight gradients are accumulated
 // in REGISTERS across all tiles of a CTA and flushed once (a few million REDs per call instead of 15 k per tile).
 // tiny-cuda-nn's fp16 rounding points are reproduced: table in half, per-corner __hfma2 accumulation,
 // dL/dy -> half, x128, per-corner half product. Deviation: the table gradient accumulates in fp32 RED
-// (the reference: fp16 atomics). This file: decoder arithmetic as fp32 FMA on the CUDA cores (mlp_mode 0); the tcgen05
+// (the reference: fp16 atomics). This file: decoder arithmetic as fp32 FMA on the CUDA cores (mlp_mode 0); the tensor-core
 // kernels (mlp_mode 1) are in sdf_tc.cu.
 #include <cuda_bf16.h>
 #include "sdf_grid.cuh"
@@ -491,7 +491,7 @@ extern "C" int gssdf_sdf_fwd(const gssdf_sdf_fwd_args *a, gssdf_stream_t stream)
     const GridGeom g = make_grid(a->net);
     GSSDF_REQUIRE(a->n_variants == 0 || a->n_variants == 1 || a->n_variants == 7, GSSDF_EINVAL, "sdf_fwd: n_variants must be 1 or 7");
     if (a->net.mlp_mode == 1) {
-        GSSDF_REQUIRE(a->net.hidden_dim == 64, GSSDF_EUNSUPPORTED, "sdf_fwd: the tcgen05 decoder needs hidden_dim 64");
+        GSSDF_REQUIRE(a->net.hidden_dim == 64, GSSDF_EUNSUPPORTED, "sdf_fwd: the tensor-core decoder needs hidden_dim 64");
         return gssdf_sdf_fwd_tc_launch(a, &g, stream);
     }
     GSSDF_REQUIRE(a->net.mlp_mode == 0, GSSDF_EINVAL, "sdf_fwd: mlp_mode must be 0 or 1");
@@ -519,12 +519,12 @@ extern "C" int gssdf_sdf_bwd(const gssdf_sdf_bwd_args *a, gssdf_stream_t stream)
     const GridGeom g = make_grid(a->net);
     GSSDF_REQUIRE(a->n_variants == 0 || a->n_variants == 1 || a->n_variants == 7, GSSDF_EINVAL, "sdf_bwd: n_variants must be 1 or 7");
     if (a->net.mlp_mode == 1) {
-        GSSDF_REQUIRE(a->net.hidden_dim == 64, GSSDF_EUNSUPPORTED, "sdf_bwd: the tcgen05 decoder needs hidden_dim 64");
+        GSSDF_REQUIRE(a->net.hidden_dim == 64, GSSDF_EUNSUPPORTED, "sdf_bwd: the tensor-core decoder needs hidden_dim 64");
         return gssdf_sdf_bwd_tc_launch(a, &g, stream);
     }
     GSSDF_REQUIRE(a->net.mlp_mode == 0, GSSDF_EINVAL, "sdf_bwd: mlp_mode must be 0 or 1");
     const int64_t n_tiles = (a->n * (a->n_variants > 1 ? a->n_variants : 1) + 63) / 64;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms * 1);  // persistent: one CTA per SM (176 KB of shared memory each)

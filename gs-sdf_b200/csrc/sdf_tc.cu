@@ -1,5 +1,5 @@
-// a9-a12 on the 5th-generation tensor cores (gssdf_sdf_net.mlp_mode == 1): the SDF decoder's dense 64-wide layers, forward AND
-// backward, as hand-written tcgen05.mma (kind::f16, bf16 inputs, fp32 accumulation in TMEM), hidden_dim 64.
+// a9-a12 on the Hopper tensor cores (gssdf_sdf_net.mlp_mode == 1): the SDF decoder's dense 64-wide layers, forward AND
+// backward, as hand-written wgmma.mma_async (bf16 operands in shared memory, fp32 accumulation in registers), hidden_dim 64.
 //
 // Reference behaviour: the decoder is torch::nn::Sequential(Linear+ReLU x (1+geo_num_layer), Linear -> 2) in fp32
 // (include/neural_net/local_map.cpp:29-42,87-103); encoding as in sdf_grid.cuh.
@@ -15,13 +15,12 @@
 // kept as two interleaved parts, byte offset of (r, k, part) = (r/8)*G + part*P + (k/8)*128 + (r%8)*16 + (k%8)*2 :
 //   as a K-major operand  (rows = M or N, k = K)    : start = base + part*P, LBO = 128, SBO = G
 //   as an MN-major operand (k = M or N, rows = K)   : start = base + part*P, SBO = 128, LBO = G
-//   as an MN-major operand with the parts STACKED along M (M = 64 hi + 64 mid = 128 when P = 1024): start = base, SBO = 128, LBO = G
-// The stacked form turns the weight-gradient GEMM dW^T[k][o] = sum_p a[p][k] g[p][o] (M = 64 otherwise) into an M = 128 UMMA whose
-// rows 0-63 / 64-127 hold the hi / mid contributions; two instructions per K step (B = g_hi, g_mid) give the full 4-term
-// product, and the halves are added when the accumulator is read out ONCE at the end of the persistent kernel (the dW accumulators
-// stay in TMEM across all tiles of a CTA: 4 x 64 columns).
+// A wgmma covers 64 rows per warpgroup, so a 128-point tile is split between warpgroups by rows (and in the backward also by 32-column
+// halves). The weight-gradient GEMM dW^T[k][o] = sum_p a[p][k] g[p][o] is an M = 64 wgmma with A = a (MN-major) and B = g (MN-major);
+// four instructions per K step (a_hi, a_mid x g_hi, g_mid) give the 4-term product. Each hidden layer's dW accumulator belongs to one
+// warpgroup and stays in its registers across all tiles of the persistent CTA; it is read out ONCE at the end.
 // Weights are pre-split once per optimiser step (gssdf_sdf_mlp_pack) into that layout (G = 3072: hi | mid | lo) and fetched per
-// layer with one 24 KiB cp.async.bulk (TMA) issued by the MMA thread; completion on an mbarrier.
+// layer with one 24 KiB cp.async.bulk (TMA) issued by one thread; completion on an mbarrier.
 #include "sdf_grid.cuh"
 #include "sdf_loss.cuh"
 
@@ -48,28 +47,55 @@ __device__ __host__ __forceinline__ uint32_t off_w(int o, int k, int part) {
     return (uint32_t)((o >> 3) * kGW + part * 1024 + (k >> 3) * 128 + (o & 7) * 16 + (k & 7) * 2);
 }
 
-// shared-memory matrix descriptor, no swizzle (layout_type 0), Blackwell descriptor version 1
+// wgmma shared-memory matrix descriptor, no swizzle (layout type 0 in bits [62,64)), base offset 0
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);  // start address, bits [0,14)
     d |= (uint64_t)(lbo >> 4) << 16;          // leading byte offset, bits [16,30): K-major: between the two 8-column cores of a K step;
                                               //   MN-major: between 8-row K groups
     d |= (uint64_t)(sbo >> 4) << 32;          // stride byte offset, bits [32,46): between 8-row (K-major) / 8-column (MN-major) M/N groups
-    d |= (uint64_t)1 << 46;
     return d;
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving reads of an accumulator above the wait for the asynchronous MMAs that write it
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x N] (+)= A . B, bf16 operands, fp32 accumulator; TA / TB = 1: that operand is MN-major. Thread t of the warpgroup holds
+// element e = 4j + 2i + c of D at row 16 (t / 32) + (t % 32) / 4 + 8i, column 8j + 2 (t % 4) + c.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {  // N = 32
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, %19, %20;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB)
         : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {  // N = 64
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(accumulate), "n"(TA), "n"(TB)
+        : "memory");
 }
 __device__ __forceinline__ bool mbar_wait_bounded(uint64_t *bar, uint32_t parity) {
     for (int it = 0; it < (1 << 24); ++it) {
@@ -86,28 +112,6 @@ __device__ __forceinline__ bool mbar_wait_bounded(uint64_t *bar, uint32_t parity
         if (ok) return true;
     }
     return false;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t v[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, "
-        "%19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t v[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 __device__ __forceinline__ void split2(float x, __nv_bfloat16 &hi, __nv_bfloat16 &mid) {
@@ -142,6 +146,23 @@ __device__ __forceinline__ void load8_sum(const unsigned char *buf, int r, int k
 #pragma unroll
     for (int e = 0; e < 8; ++e) x[e] = __bfloat162float(hp[e]) + __bfloat162float(mp[e]);
 }
+// columns k0, k0 + 1 (k0 even) of row r: the accumulator-fragment counterparts of store8 / load8_hi
+__device__ __forceinline__ void store2(unsigned char *buf, unsigned char *lo_buf, int r, int k0, float x0, float x1) {
+    __nv_bfloat16 h0, m0, l0, h1, m1, l1;
+    split3(x0, h0, m0, l0);
+    split3(x1, h1, m1, l1);
+    *reinterpret_cast<__nv_bfloat162 *>(buf + off_act(r, k0, 0)) = __halves2bfloat162(h0, h1);
+    *reinterpret_cast<__nv_bfloat162 *>(buf + off_act(r, k0, 1)) = __halves2bfloat162(m0, m1);
+    if (lo_buf) *reinterpret_cast<__nv_bfloat162 *>(lo_buf + off_lo(r, k0)) = __halves2bfloat162(l0, l1);
+}
+__device__ __forceinline__ float2 load2_hi(const unsigned char *buf, int r, int k0) {
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(buf + off_act(r, k0, 0)));
+}
+// sum over the 4 lanes of a quad (the lanes that share an accumulator row)
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 // sum each of 16 per-thread values over the 32 lanes of the warp: 8+4+2+1 exchange steps + one xor-16; every lane ends with the
 // total of column (lane & 15)
 __device__ __forceinline__ float colsum16(float c[16], int lane) {
@@ -157,43 +178,36 @@ __device__ __forceinline__ float colsum16(float c[16], int lane) {
     return c[0] + __shfl_xor_sync(0xffffffffu, c[0], 16);
 }
 
-// instruction descriptor: D = F32 (bit 4), A = B = BF16 (bits 7, 10), N = 64 (N >> 3 at bit 17), M = 128 (M >> 4 at bit 24)
-constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-constexpr uint32_t kIdescBmn = kIdesc | (1u << 16);                 // B MN-major
-constexpr uint32_t kIdescAmnBmn = kIdesc | (1u << 15) | (1u << 16);  // A and B MN-major
-
-// forward layer l on the tensor cores (issued by one thread): D[128 x 64] = A_l . W_l^T with the 3-term split
-//   l == 0: A = encoded features (fp16 values: hi + mid is exact, no lo), K = 32, layout off_feat
-//   l >= 1: A = hi/mid in `a_base` (off_act) + lo in `lo_base` (off_lo), K = 64
-__device__ __forceinline__ void issue_forward_layer(uint32_t tmD, int l, uint32_t a_base, uint32_t lo_base, uint32_t w_base) {
-    uint32_t acc = 0;
-    if (l == 0) {
-        for (int ks = 0; ks < kFeat / 16; ++ks) {
-            const uint32_t ko = ks * 256;
-            const uint64_t ah = make_desc(a_base + ko, 128, kGA0), am = make_desc(a_base + 512 + ko, 128, kGA0);
-            const uint64_t wh = make_desc(w_base + ko, 128, kGW), wm = make_desc(w_base + 1024 + ko, 128, kGW),
-                           wl = make_desc(w_base + 2048 + ko, 128, kGW);
-            umma_bf16(tmD, ah, wh, kIdesc, acc); acc = 1;
-            umma_bf16(tmD, ah, wm, kIdesc, 1);
-            umma_bf16(tmD, am, wh, kIdesc, 1);
-            umma_bf16(tmD, am, wm, kIdesc, 1);
-            umma_bf16(tmD, ah, wl, kIdesc, 1);
-        }
-    } else {
-        for (int ks = 0; ks < 64 / 16; ++ks) {
-            const uint32_t ko = ks * 256;
-            const uint64_t ah = make_desc(a_base + ko, 128, kGA), am = make_desc(a_base + 1024 + ko, 128, kGA),
-                           al = make_desc(lo_base + ko, 128, kGL);
-            const uint64_t wh = make_desc(w_base + ko, 128, kGW), wm = make_desc(w_base + 1024 + ko, 128, kGW),
-                           wl = make_desc(w_base + 2048 + ko, 128, kGW);
-            umma_bf16(tmD, ah, wh, kIdesc, acc); acc = 1;
-            umma_bf16(tmD, ah, wm, kIdesc, 1);
-            umma_bf16(tmD, am, wh, kIdesc, 1);
-            umma_bf16(tmD, am, wm, kIdesc, 1);
-            umma_bf16(tmD, ah, wl, kIdesc, 1);
-            umma_bf16(tmD, al, wh, kIdesc, 1);
+// forward layer on the tensor cores (issued by one warpgroup, committed as one group): D[64 x N] = A . W^T with the 3-term split, or
+// the 2-term split (hh hm mh mm) when THREE is false. a_base / lo_base point at the warpgroup's 64 rows, w_base at its N outputs.
+//   FEAT : A = encoded features (fp16 values: hi + mid is exact, no lo), K = 32, layout off_feat
+//   else : A = hi/mid in `a_base` (off_act) + lo in `lo_base` (off_lo), K = 64
+// Straight-line code between fence and commit (compile-time choices, unrolled K loop): a branch inside an MMA sequence makes ptxas
+// serialise the wgmma chain.
+template <bool FEAT, bool THREE, int R>
+__device__ __forceinline__ void issue_layer(float (&d)[R], uint32_t a_base, uint32_t lo_base, uint32_t w_base) {
+    constexpr uint32_t ga = FEAT ? kGA0 : kGA, am = FEAT ? 512u : 1024u;
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < (FEAT ? kFeat : 64) / 16; ++ks) {
+        const uint32_t ko = ks * 256;
+        const uint64_t ah = make_desc(a_base + ko, 128, ga), amd = make_desc(a_base + am + ko, 128, ga);
+        const uint64_t wh = make_desc(w_base + ko, 128, kGW), wm = make_desc(w_base + 1024 + ko, 128, kGW);
+        wgmma_bf16<0, 0>(d, ah, wh, ks > 0 ? 1u : 0u);
+        wgmma_bf16<0, 0>(d, ah, wm, 1);
+        wgmma_bf16<0, 0>(d, amd, wh, 1);
+        wgmma_bf16<0, 0>(d, amd, wm, 1);
+        if constexpr (THREE) {
+            wgmma_bf16<0, 0>(d, ah, make_desc(w_base + 2048 + ko, 128, kGW), 1);
+            if constexpr (!FEAT) wgmma_bf16<0, 0>(d, make_desc(lo_base + ko, 128, kGL), wh, 1);
         }
     }
+    wg_commit();
+}
+template <bool THREE = true, int R>
+__device__ __forceinline__ void issue_forward_layer(float (&d)[R], int l, uint32_t a_base, uint32_t lo_base, uint32_t w_base) {
+    if (l == 0) issue_layer<true, THREE>(d, a_base, lo_base, w_base);
+    else issue_layer<false, THREE>(d, a_base, lo_base, w_base);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -218,8 +232,8 @@ __global__ void __launch_bounds__(256) mlp_pack_kernel(const float *__restrict__
 
 // ---------------------------------------------------------------------------------------------
 // forward: persistent CTAs (two per SM) walk the 128-point tiles. The layout stride n is a CAPACITY (the live count is a device value), so
-// most tiles of a launch can be dead: a dead tile costs one loop iteration here instead of a CTA launch, and TMEM allocation, barrier
-// initialisation and the bias loads happen once per CTA instead of once per tile.
+// most tiles of a launch can be dead: a dead tile costs one loop iteration here instead of a CTA launch, and barrier initialisation
+// and the bias loads happen once per CTA instead of once per tile. Warpgroup wg computes rows 64 wg .. 64 wg + 63 of each tile.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kFwdTcThreads)
 sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles) {
@@ -231,25 +245,18 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
     unsigned char *sW = sL + 16 * kGL;           // 24 KB weight image of the current layer
     float *s_bias = reinterpret_cast<float *>(sW + kWImg);  // [5][64]
     float *s_wout = s_bias + 5 * 64;             // [2][64] + [2]
-    float *s_part = s_wout + 132;                // [2 column halves][128][2]
-    __shared__ __align__(8) uint64_t s_mbar[2];  // [0] MMA commit, [1] weight copy
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_wbar;     // weight copy
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, h = warp >> 2, row = 32 * q + lane;
+    const int wg = warp >> 2, fr = 64 * wg + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);  // accumulator fragment origin
     const int nh = 1 + a.net.n_hidden;
     const int64_t n_eval = a.n * max(a.n_variants, 1);
     const int64_t n_live = a.n_live ? min((int64_t)*a.n_live, a.n) : a.n;
     const __half2 *table = reinterpret_cast<const __half2 *>(a.net.table_half);
     const unsigned char *wimg = reinterpret_cast<const unsigned char *>(a.net.mlp_packed);
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "n"(64));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     if (tid == 0) {
-        mbar_init(&s_mbar[0], 1);
-        mbar_init(&s_mbar[1], 1);
+        mbar_init(&s_wbar, 1);
         fence_mbar_init();
     }
     {
@@ -261,20 +268,17 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
         }
         for (int e = tid; e < 2 * HID + 2; e += kFwdTcThreads) s_wout[e] = __ldg(W + e);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = s_tmem;
     bool ok = true;
-    uint32_t done_layers = 0;  // layers completed by this CTA so far: both barriers complete one phase per layer
+    uint32_t done_layers = 0;  // layers completed by this CTA so far: the weight barrier completes one phase per layer
     for (int64_t tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
     const int64_t base = tile * TM;
     if (base % a.n >= n_live && base % a.n + TM <= a.n) continue;  // CTA-uniform: the whole tile is beyond the live rows
     if (a.skip_base_variant && base + TM <= a.n) continue;           // CTA-uniform: only variant-0 evaluations in this tile
     const int tm = (int)min((int64_t)TM, n_eval - base);
-    if (tid == 0) {  // the previous tile's MMAs are complete (its last commit was waited for): sW is free
-        mbar_arrive_expect_tx(&s_mbar[1], kWImg);
-        bulk_g2s(sW, wimg, kWImg, &s_mbar[1]);
+    if (tid == 0) {  // the previous tile's MMAs are complete (every warpgroup waited for them before the last barrier): sW is free
+        mbar_arrive_expect_tx(&s_wbar, kWImg);
+        bulk_g2s(sW, wimg, kWImg, &s_wbar);
     }
     // 1. encode: 128 points x 16 levels -> features (global, optional) + A operand of layer 0. Branch-free batches of 4 (point,
     //    level) tasks per thread so that 32 table gathers are in flight before the first one is consumed.
@@ -301,57 +305,47 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
         }
     }
     for (int l = 0; l < nh; ++l) {
-        const uint32_t parity = (done_layers + (uint32_t)l) & 1u;
         fence_proxy_async();  // generic-proxy writes of the A operand -> visible to the tensor core
-        __syncthreads();
-        if (tid == 0) {
-            ok = mbar_wait_bounded(&s_mbar[1], parity);  // W_l has landed
-            tc_fence_after();
-            if (ok) issue_forward_layer(tmem, l, smem_u32(l == 0 ? sF : sA), smem_u32(sL), smem_u32(sW));
-            umma_commit(&s_mbar[0]);
-        }
-        ok = mbar_wait_bounded(&s_mbar[0], parity) && ok;
+        ok = __syncthreads_and(mbar_wait_bounded(&s_wbar, (done_layers + (uint32_t)l) & 1u));  // W_l has landed
         if (!ok) break;
-        tc_fence_after();
-        if (tid == 0 && l + 1 < nh) {  // the MMAs are done with sW: fetch the next layer while the epilogue runs
-            mbar_arrive_expect_tx(&s_mbar[1], kWImg);
-            bulk_g2s(sW, wimg + (size_t)(l + 1) * kWImg, kWImg, &s_mbar[1]);
+        float d[32];
+        issue_forward_layer(d, l, smem_u32(l == 0 ? sF + 8 * wg * kGA0 : sA + 8 * wg * kGA), smem_u32(sL + 8 * wg * kGL), smem_u32(sW));
+        wg_wait();
+        acc_fence(d);
+        __syncthreads();  // every warpgroup's MMAs are done with sW: fetch the next layer while the epilogue runs
+        if (tid == 0 && l + 1 < nh) {
+            mbar_arrive_expect_tx(&s_wbar, kWImg);
+            bulk_g2s(sW, wimg + (size_t)(l + 1) * kWImg, kWImg, &s_wbar);
         }
-        uint32_t v[32];
-        tmem_ld32(tmem + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * h), v);
         float act[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) act[j] = fmaxf(__uint_as_float(v[j]) + s_bias[l * 64 + 32 * h + j], 0.f);
-        if (l < nh - 1) {
+        for (int e = 0; e < 32; ++e) act[e] = fmaxf(d[e] + s_bias[l * 64 + 8 * (e >> 2) + fc + (e & 1)], 0.f);
+        if (l < nh - 1) {  // rows of this warpgroup only: sA is rewritten in place
 #pragma unroll
-            for (int jj = 0; jj < 4; ++jj) store8(sA, sL, row, 32 * h + jj * 8, act + jj * 8);
-        } else {  // output layer (64 -> 2) on the CUDA cores, straight from the registers
-            float p0 = 0.f, p1 = 0.f;
+            for (int e = 0; e < 32; e += 2) store2(sA, sL, fr + 8 * ((e >> 1) & 1), 8 * (e >> 2) + fc, act[e], act[e + 1]);
+        } else {  // output layer (64 -> 2) on the CUDA cores, straight from the registers; a quad holds a whole row
+            float p0[2] = {0.f, 0.f}, p1[2] = {0.f, 0.f};
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                p0 = fmaf(act[j], s_wout[32 * h + j], p0);
-                p1 = fmaf(act[j], s_wout[HID + 32 * h + j], p1);
+            for (int e = 0; e < 32; ++e) {
+                const int i = (e >> 1) & 1, c = 8 * (e >> 2) + fc + (e & 1);
+                p0[i] = fmaf(act[e], s_wout[c], p0[i]);
+                p1[i] = fmaf(act[e], s_wout[HID + c], p1[i]);
             }
-            s_part[(h * TM + row) * 2] = p0;
-            s_part[(h * TM + row) * 2 + 1] = p1;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const float s0 = quad_sum(p0[i]), s1 = quad_sum(p1[i]);
+                const int p = fr + 8 * i;
+                if ((lane & 3) == 0 && p < tm && (base + p) % a.n < n_live) {
+                    a.sdf[base + p] = s0 + s_wout[2 * HID];
+                    if (a.y1) a.y1[base + p] = s1 + s_wout[2 * HID + 1];
+                }
+            }
         }
-        tc_fence_before();
     }
     done_layers += (uint32_t)nh;
-    ok = __syncthreads_and(ok);  // (thread 0's barrier waits decide for the CTA)
-    if (ok && tid < TM) {
-        const int p = tid;
-        if (p < tm && (base + p) % a.n < n_live) {
-            a.sdf[base + p] = s_part[p * 2] + s_part[(TM + p) * 2] + s_wout[2 * HID];
-            if (a.y1) a.y1[base + p] = s_part[p * 2 + 1] + s_part[(TM + p) * 2 + 1] + s_wout[2 * HID + 1];
-        }
-    }
-    __syncthreads();  // s_part / sF / sA are rewritten by the next tile
+    __syncthreads();  // sF / sA are rewritten by the next tile
     }  // tile loop
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(64));
-    if (!ok) __trap();  // the tensor core / copy engine never signalled: fail loudly rather than return garbage
+    if (!ok) __trap();  // the copy engine never signalled: fail loudly rather than return garbage
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -359,7 +353,7 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
 // ---------------------------------------------------------------------------------------------
 // Shared-memory budget: the SM's 256 KiB are split between shared memory and L1, and the carve-out comes in steps (.., 196, 228 KiB).
 // Staying under 196 KiB per CTA (incl. 1 KiB system reserve) keeps a 60 KiB L1 for the hash-grid gathers; at 228 KiB only 28 KiB
-// remain and the kernel ran 20 % slower. Both variants are sized to fit the 196 KiB step.
+// would remain. Both variants are sized to fit the 196 KiB step.
 constexpr size_t kBwdTcMain = 16 * kGA0 + 3 * 16 * kGA + 16 * kGA + 16 * kGL + kWImg;
 constexpr size_t kBwdTcMisc = sizeof(float) * (4 * 64 + 132 + 384 + 4 * 128);                    // bias, w_out, dx|seed, column sums
 constexpr size_t kBwdTcMiscAnalytic = 128 * 16 * sizeof(uint16_t) + 128 * 3 * sizeof(float) + 64;  // ReLU masks, numerical gradient, tile bases
@@ -400,11 +394,14 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
     uint16_t *s_mask16 = reinterpret_cast<uint16_t *>(s_col + 4 * 128);  // ANALYTIC only: [128 slots][4 layers][4 column quarters] ReLU masks
     float *s_gnum = s_col + 4 * 128 + 1024;      // ANALYTIC only: [128][3] numerical gradient of the pending points (align loss)
     int64_t *s_tbase = reinterpret_cast<int64_t *>(s_gnum + 384);  // ANALYTIC only: first point of each tile of the pending batch [8]
-    __shared__ __align__(8) uint64_t s_mbar[2];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_wbar;     // weight copy
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, cq = warp >> 2, row = 32 * q + lane, col0 = 16 * cq;  // epilogue role: TMEM lanes 32q.., columns 16cq..
+    const int q = warp & 3, cq = warp >> 2, row = 32 * q + lane, col0 = 16 * cq;  // CUDA-core role: row 32q + lane, columns 16cq..
+    // tensor-core role: warpgroup wg computes the rows 64 (wg & 1) .. x columns 32 (wg >> 1) .. of every [128 x 64] D (m64n32), and owns
+    // the weight-gradient accumulator of layer wg (m64n64, rows k, columns o)
+    const int wg = warp >> 2, fr = 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);
+    const int dr = 64 * (wg & 1) + fr, dc = 32 * (wg >> 1) + fc;  // D fragment origin
     const int nh = 1 + a.net.n_hidden;
     const int64_t n_eval = a.n * max(a.n_variants, 1);
     const int64_t n_live = a.n_live ? min((int64_t)*a.n_live, a.n) : a.n;
@@ -417,13 +414,8 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
     float acc2_wo = 0.f;  // second-order gradient of w_out[0] (thread (q == 0, lane < 16) owns column 16cq + lane)
     int n_coll = 0;       // base points waiting for the second-order phase (slots 0 .. n_coll-1 of s_mask16 / s_cpt / s_gnum)
 
-    if (warp == 0) {  // TMEM: D (64 columns) + one 64-column weight-gradient accumulator per hidden layer -> 512-column allocation
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     if (tid == 0) {
-        mbar_init(&s_mbar[0], 1);
-        mbar_init(&s_mbar[1], 1);
+        mbar_init(&s_wbar, 1);
         fence_mbar_init();
     }
     {
@@ -435,14 +427,65 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
         }
         for (int e = tid; e < 2 * HID + 2; e += NT) s_wout[e] = __ldg(W + e);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = s_tmem, tmD = tmem, tmW = tmem + 64;
-    uint32_t ph_mma = 0, ph_w = 0;  // mbarrier phases (ph_w is only meaningful in thread 0)
+    uint32_t ph_w = 0;  // weight-barrier phase (every thread waits)
     bool ok = true, first_tile = true;
     float dbias[4] = {0.f, 0.f, 0.f, 0.f};  // thread (q == 0, lane < 16) owns column 16cq + lane of every hidden layer's bias gradient
     float dwo0 = 0.f, dwo1 = 0.f, dbo = 0.f;
+    float accW[32];  // dW_wg^T [64 k][64 o] of the layer this warpgroup owns, summed over all tiles of the CTA
+#pragma unroll
+    for (int e = 0; e < 32; ++e) accW[e] = 0.f;
+    float dD[16];    // this thread's fragment of the current D
+
+    // every thread waits for the weight image (if asked), then the CTA barrier makes the A / B operands visible to the tensor core
+    auto sync_w = [&](bool wait) {
+        fence_proxy_async();
+        bool landed = true;
+        if (wait) { landed = mbar_wait_bounded(&s_wbar, ph_w); ph_w ^= 1; }
+        ok = __syncthreads_and(landed) && ok;
+    };
+    auto load_w = [&](int l) {  // thread 0
+        mbar_arrive_expect_tx(&s_wbar, kWImg);
+        bulk_g2s(sW, wimg + (size_t)l * kWImg, kWImg, &s_wbar);
+    };
+    auto finish = [&]() {  // wait for this warpgroup's MMAs, then for everyone's: sG / sW are free to be rewritten
+        wg_wait();
+        acc_fence(dD);
+        __syncthreads();
+    };
+    // D[p][k] = sum_o G[p][o] W[o][k]: A = sG (K-major), B = the weight image (MN-major: N = k, K = o)
+    auto issue_gw = [&]() {
+        const uint32_t gB = smem_u32(sG) + 8 * (wg & 1) * kGA, wB = smem_u32(sW) + 4 * (wg >> 1) * 128;
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < HID / 16; ++ks) {
+            const uint64_t gh = make_desc(gB + ks * 256, 128, kGA), gm = make_desc(gB + 1024 + ks * 256, 128, kGA);
+            const uint64_t wh = make_desc(wB + ks * 2 * kGW, kGW, 128), wm = make_desc(wB + 1024 + ks * 2 * kGW, kGW, 128);
+            wgmma_bf16<0, 1>(dD, gh, wh, ks > 0 ? 1u : 0u);
+            wgmma_bf16<0, 1>(dD, gh, wm, 1);
+            wgmma_bf16<0, 1>(dD, gm, wh, 1);
+            wgmma_bf16<0, 1>(dD, gm, wm, 1);
+        }
+        wg_commit();
+    };
+    // dW_l^T[k][o] += sum_p A[p][k] G[p][o] on the warpgroup that owns layer l: A = a_l (or q_l) where the forward keeps a_l, B = sG, both
+    // MN-major, K = points. For l == 0 the 64 rows of the M = 64 view run past the 32 features (finite bf16 data, rows ignored).
+    auto issue_dw = [&](int l) {
+        if (wg != l) return;
+        const uint32_t aB = smem_u32(l == 0 ? sF : sAct + (l - 1) * 16 * kGA), ga = l == 0 ? kGA0 : kGA, am = l == 0 ? 512u : 1024u;
+        const uint32_t gB = smem_u32(sG);
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < TM / 16; ++ks) {
+            const uint64_t ah = make_desc(aB + ks * 2 * ga, ga, 128), amd = make_desc(aB + am + ks * 2 * ga, ga, 128);
+            const uint64_t gh = make_desc(gB + ks * 2 * kGA, kGA, 128), gm = make_desc(gB + 1024 + ks * 2 * kGA, kGA, 128);
+            wgmma_bf16<1, 1>(accW, ah, gh, 1);
+            wgmma_bf16<1, 1>(accW, ah, gm, 1);
+            wgmma_bf16<1, 1>(accW, amd, gh, 1);
+            wgmma_bf16<1, 1>(accW, amd, gm, 1);
+        }
+        wg_commit();
+    };
 
 
     // ---- second-order phase (ANALYTIC): gradient of the eikonal / align losses -- functions of g = d sdf / d x -- w.r.t. decoder and
@@ -451,7 +494,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
     //        g = dy_dx^T half(dfeat) (tcnn rounding points); c = dL/dg; r = half(dy_dx c); table: encode_level_bwd2
     //        q-chain  q_0 = r; q_{l+1} = D_{l+1} (.) (q_l W_l^T)                                   (forward-like, no bias)
     //        dL/dW_l += u_{l+1} (x) q_l  : the SAME stacked dW GEMM, A = q_l parked where a_l lives, B = u_{l+1} where g_l lives,
-    //        accumulating into the same TMEM tiles as the first-order weight gradient; dL/dw_out[0] += colsum(q_nh); no bias terms.
+    //        accumulating into the same registers as the first-order weight gradient; dL/dw_out[0] += colsum(q_nh); no bias terms.
     //      The u-chain runs twice (first to get dfeat, then again to pair u_{l+1} with the stored q_l) so that only one gradient
     //      buffer is live. ReLU masks D_l come from the bit masks captured in the forward epilogues.
     auto second_order = [&]() {
@@ -471,57 +514,34 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
             store8(sG, nullptr, row, col0, u);
             store8(sG, nullptr, row, col0 + 8, u + 8);
         };
-        auto load_w = [&](int l) {  // thread 0
-            mbar_arrive_expect_tx(&s_mbar[1], kWImg);
-            bulk_g2s(sW, wimg + (size_t)l * kWImg, kWImg, &s_mbar[1]);
+        // bit of D fragment element e in the slot's 16-column mask word (column 16 cq' + 8 (j & 1) + fc + c, cq' = 2 (wg >> 1) + j / 2)
+        auto mask_bit = [&](int slot, int l, int e) -> bool {
+            const int j = e >> 2;
+            return (s_mask16[(slot * 4 + l - 1) * 4 + 2 * (wg >> 1) + (j >> 1)] >> (8 * (j & 1) + fc + (e & 1))) & 1u;
         };
-        auto issue_d = [&]() {  // D = G . W (A = sG K-major, B = weight image MN-major), thread 0
-            const uint32_t gB = smem_u32(sG), wB = smem_u32(sW);
-            uint32_t acc = 0;
-            for (int ks = 0; ks < HID / 16; ++ks) {
-                const uint64_t gh = make_desc(gB + ks * 256, 128, kGA), gm = make_desc(gB + 1024 + ks * 256, 128, kGA);
-                const uint64_t wh = make_desc(wB + ks * 2 * kGW, kGW, 128), wm = make_desc(wB + 1024 + ks * 2 * kGW, kGW, 128);
-                umma_bf16(tmD, gh, wh, kIdescBmn, acc); acc = 1;
-                umma_bf16(tmD, gh, wm, kIdescBmn, 1);
-                umma_bf16(tmD, gm, wh, kIdescBmn, 1);
-                umma_bf16(tmD, gm, wm, kIdescBmn, 1);
+        auto mask_store = [&](int l, unsigned char *dst) {  // dst = D_l (.) D, from this thread's D fragment   (l = 1..nh)
+#pragma unroll
+            for (int e = 0; e < 16; e += 2) {
+                const int r = dr + 8 * ((e >> 1) & 1);
+                store2(dst, nullptr, r, dc + 8 * (e >> 2), mask_bit(r, l, e) ? dD[e] : 0.f, mask_bit(r, l, e + 1) ? dD[e + 1] : 0.f);
             }
         };
-        auto mask_store = [&](int l, unsigned char *dst) {  // dst[row][cols] = D_l (.) TMEM D   (l = 1..nh)
-            uint32_t v[16];
-            tmem_ld16(tmD + ((uint32_t)(32 * q) << 16) + (uint32_t)col0, v);
-            const uint32_t bits = s_mask16[(row * 4 + l - 1) * 4 + cq];
-            float o[16];
+        auto store_gf = [&]() {  // dfeat (columns 0..31 of D) in fp32
+            if (wg >> 1) return;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) o[j] = ((bits >> j) & 1u) ? __uint_as_float(v[j]) : 0.f;
-            store8(dst, nullptr, row, col0, o);
-            store8(dst, nullptr, row, col0 + 8, o + 8);
+            for (int e = 0; e < 16; ++e) gf[(dr + 8 * ((e >> 1) & 1)) * 33 + dc + 8 * (e >> 2) + (e & 1)] = dD[e];
         };
         // -- u-chain, pass 1: dfeat
         seed_u();
         if (tid == 0) { fence_proxy_async(); load_w(nh - 1); }
         for (int l = nh - 1; l >= 0 && ok; --l) {
-            fence_proxy_async();
-            __syncthreads();
-            if (tid == 0) {
-                ok = mbar_wait_bounded(&s_mbar[1], ph_w); ph_w ^= 1;
-                tc_fence_after();
-                if (ok) issue_d();
-                umma_commit(&s_mbar[0]);
-            }
-            ok = mbar_wait_bounded(&s_mbar[0], ph_mma) && ok; ph_mma ^= 1;
+            sync_w(true);
             if (!ok) return;
-            tc_fence_after();
+            issue_gw();
+            finish();
             if (tid == 0 && l > 0) load_w(l - 1);
-            if (l > 0) {
-                mask_store(l, sG);
-            } else if (cq < 2) {
-                uint32_t v[16];
-                tmem_ld16(tmD + ((uint32_t)(32 * q) << 16) + (uint32_t)col0, v);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) gf[row * 33 + col0 + j] = __uint_as_float(v[j]);
-            }
-            tc_fence_before();
+            if (l > 0) mask_store(l, sG);
+            else store_gf();
         }
         __syncthreads();
         // -- pass A: g (x01 units) = tcnn input gradient with cotangent dfeat, summed over the levels
@@ -588,78 +608,47 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
         }
         if (!a.mlp_grad) { __syncthreads(); return; }
         // -- q-chain (forward-like, 2-term split, no bias): q_l parked where the forward keeps a_l
+        __syncthreads();  // pass B has read all of dfeat, whose last rows spill into sW, before the weight copy overwrites sW
         if (tid == 0) { fence_proxy_async(); load_w(0); }
         for (int l = 0; l < nh; ++l) {
-            fence_proxy_async();
-            __syncthreads();
-            if (tid == 0) {
-                ok = mbar_wait_bounded(&s_mbar[1], ph_w); ph_w ^= 1;
-                tc_fence_after();
-                if (ok) {
-                    const uint32_t aB = smem_u32(l == 0 ? sF : sAct + (l - 1) * 16 * kGA), wB = smem_u32(sW);
-                    const uint32_t ga = l == 0 ? kGA0 : kGA, am = l == 0 ? 512u : 1024u;
-                    uint32_t acc = 0;
-                    for (int ks = 0; ks < (l == 0 ? kFeat : HID) / 16; ++ks) {
-                        const uint32_t ko = ks * 256;
-                        const uint64_t ah = make_desc(aB + ko, 128, ga), amd = make_desc(aB + am + ko, 128, ga);
-                        const uint64_t wh = make_desc(wB + ko, 128, kGW), wm = make_desc(wB + 1024 + ko, 128, kGW);
-                        umma_bf16(tmD, ah, wh, kIdesc, acc); acc = 1;
-                        umma_bf16(tmD, ah, wm, kIdesc, 1);
-                        umma_bf16(tmD, amd, wh, kIdesc, 1);
-                        umma_bf16(tmD, amd, wm, kIdesc, 1);
-                    }
-                }
-                umma_commit(&s_mbar[0]);
-            }
-            ok = mbar_wait_bounded(&s_mbar[0], ph_mma) && ok; ph_mma ^= 1;
+            sync_w(true);
             if (!ok) return;
-            tc_fence_after();
+            issue_forward_layer<false>(dD, l, smem_u32(l == 0 ? sF + 8 * (wg & 1) * kGA0 : sAct + (l - 1) * 16 * kGA + 8 * (wg & 1) * kGA),
+                                       0u, smem_u32(sW) + 4 * (wg >> 1) * kGW);
+            finish();
             if (tid == 0 && (l + 1 < nh || nh > 1)) load_w(l + 1 < nh ? l + 1 : nh - 1);  // next q layer, or the first weights of the second u pass
             if (l < nh - 1) {
                 mask_store(l + 1, sAct + l * 16 * kGA);
-            } else {  // q_nh is only needed for dL/dw_out[0] = its column sums
-                uint32_t v[16];
-                tmem_ld16(tmD + ((uint32_t)(32 * q) << 16) + (uint32_t)col0, v);
-                const uint32_t bits = s_mask16[(row * 4 + nh - 1) * 4 + cq];
-                float c[16];
+            } else {  // q_nh is only needed for dL/dw_out[0] = its column sums: over the fragment's 2 rows, then the warp's 8 row pairs
 #pragma unroll
-                for (int j = 0; j < 16; ++j) c[j] = ((bits >> j) & 1u) ? __uint_as_float(v[j]) : 0.f;
-                const float sres = colsum16(c, lane);
-                if (lane < 16) s_col[q * 128 + col0 + lane] = sres;
+                for (int e = 0; e < 16; e += 4) {
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        float s = (mask_bit(dr, nh, e + c) ? dD[e + c] : 0.f) + (mask_bit(dr + 8, nh, e + 2 + c) ? dD[e + 2 + c] : 0.f);
+                        s += __shfl_xor_sync(0xffffffffu, s, 4);
+                        s += __shfl_xor_sync(0xffffffffu, s, 8);
+                        s += __shfl_xor_sync(0xffffffffu, s, 16);
+                        if (lane < 4) s_col[(4 * (wg & 1) + (warp & 3)) * 64 + dc + 2 * e + c] = s;  // [8 row groups][64]
+                    }
+                }
             }
-            tc_fence_before();
         }
         __syncthreads();
         if (q == 0 && lane < 16) {
             const int c = col0 + lane;
-            acc2_wo += s_col[c] + s_col[128 + c] + s_col[256 + c] + s_col[384 + c];
+#pragma unroll
+            for (int rg = 0; rg < 8; ++rg) acc2_wo += s_col[rg * 64 + c];
         }
         // -- u-chain, pass 2: dW_l += u_{l+1} (x) q_l on the way down
         seed_u();
         for (int l = nh - 1; l >= 0 && ok; --l) {
-            fence_proxy_async();
-            __syncthreads();
-            if (tid == 0) {
-                if (l > 0) { ok = mbar_wait_bounded(&s_mbar[1], ph_w); ph_w ^= 1; }
-                tc_fence_after();
-                if (ok) {
-                    const uint32_t gB = smem_u32(sG);
-                    const uint32_t aB = smem_u32(l == 0 ? sF : sAct + (l - 1) * 16 * kGA), ga = l == 0 ? kGA0 : kGA;
-                    for (int ks = 0; ks < TM / 16; ++ks) {
-                        const uint64_t ad = make_desc(aB + ks * 2 * ga, ga, 128);
-                        umma_bf16(tmW + 64 * l, ad, make_desc(gB + ks * 2 * kGA, kGA, 128), kIdescAmnBmn, 1);
-                        umma_bf16(tmW + 64 * l, ad, make_desc(gB + 1024 + ks * 2 * kGA, kGA, 128), kIdescAmnBmn, 1);
-                    }
-                    if (l > 0) issue_d();
-                }
-                umma_commit(&s_mbar[0]);
-            }
-            ok = mbar_wait_bounded(&s_mbar[0], ph_mma) && ok; ph_mma ^= 1;
+            sync_w(l > 0);
             if (!ok) return;
-            tc_fence_after();
+            issue_dw(l);
+            if (l > 0) issue_gw();
+            finish();
             if (tid == 0 && l > 1) load_w(l - 1);
             if (l > 0) mask_store(l, sG);
-            tc_fence_before();
         }
         __syncthreads();
     };
@@ -684,8 +673,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
         __syncthreads();  // everything of the previous tile (sL/sW as dL/dfeat, s_dx, s_seed) has been consumed
         if (tid == 0) {
             fence_proxy_async();
-            mbar_arrive_expect_tx(&s_mbar[1], kWImg);
-            bulk_g2s(sW, wimg, kWImg, &s_mbar[1]);
+            load_w(0);
         }
         // ---- 1. encode -> a_0, seeds (4 tasks per thread, branch-free: 32 gathers in flight)
         {
@@ -715,61 +703,64 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
         }
         // ---- 2. forward recompute; a_{l+1} stays in shared memory (the last one parks in sG)
         for (int l = 0; l < nh; ++l) {
-            fence_proxy_async();
-            __syncthreads();
-            if (tid == 0) {
-                ok = mbar_wait_bounded(&s_mbar[1], ph_w);
-                ph_w ^= 1;
-                tc_fence_after();
-                if (ok) issue_forward_layer(tmD, l, smem_u32(l == 0 ? sF : sAct + (l - 1) * 16 * kGA), smem_u32(sL), smem_u32(sW));
-                umma_commit(&s_mbar[0]);
-            }
-            ok = mbar_wait_bounded(&s_mbar[0], ph_mma) && ok;
-            ph_mma ^= 1;
+            sync_w(true);
             if (!ok) break;
-            tc_fence_after();
-            if (tid == 0 && l + 1 < nh) {  // (the last forward layer's weights are the first ones the backward needs: keep them)
-                mbar_arrive_expect_tx(&s_mbar[1], kWImg);
-                bulk_g2s(sW, wimg + (size_t)(l + 1) * kWImg, kWImg, &s_mbar[1]);
-            }
-            uint32_t v[16];
-            tmem_ld16(tmD + ((uint32_t)(32 * q) << 16) + (uint32_t)col0, v);
+            issue_forward_layer(dD, l, smem_u32(l == 0 ? sF + 8 * (wg & 1) * kGA0 : sAct + (l - 1) * 16 * kGA + 8 * (wg & 1) * kGA),
+                                smem_u32(sL + 8 * (wg & 1) * kGL), smem_u32(sW) + 4 * (wg >> 1) * kGW);
+            finish();
+            if (tid == 0 && l + 1 < nh) load_w(l + 1);  // (the last forward layer's weights are the first ones the backward needs: keep them)
             float act[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) act[j] = fmaxf(__uint_as_float(v[j]) + s_bias[l * 64 + col0 + j], 0.f);
+            for (int e = 0; e < 16; ++e) act[e] = fmaxf(dD[e] + s_bias[l * 64 + dc + 8 * (e >> 2) + (e & 1)], 0.f);
             unsigned char *dst = (l < nh - 1) ? sAct + l * 16 * kGA : sG;
-            store8(dst, l < nh - 1 ? sL : nullptr, row, col0, act);
-            store8(dst, l < nh - 1 ? sL : nullptr, row, col0 + 8, act + 8);
+#pragma unroll
+            for (int e = 0; e < 16; e += 2) store2(dst, l < nh - 1 ? sL : nullptr, dr + 8 * ((e >> 1) & 1), dc + 8 * (e >> 2), act[e], act[e + 1]);
             if (analytic) {  // ReLU mask of z_{l+1} of the BASE rows: kept in the pending batch for the second-order phase
-                const int jb = row / V;
-                if (row - jb * V == 0 && jb < PT && base + jb < n_live) {
-                    uint32_t bits = 0;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) bits |= (act[j] > 0.f ? 1u : 0u) << j;
-                    s_mask16[((n_coll + jb) * 4 + l) * 4 + cq] = (uint16_t)bits;
+                for (int i = 0; i < 2; ++i) {
+                    uint32_t bits[2] = {0u, 0u};  // the two 16-column words this fragment row touches; a quad completes them
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) bits[j >> 1] |= (act[4 * j + 2 * i + c] > 0.f ? 1u : 0u) << (8 * (j & 1) + fc + c);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
+                        bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
+                    }
+                    const int r = dr + 8 * i, jb = r / V;
+                    if ((lane & 3) == 0 && r - jb * V == 0 && jb < PT && base + jb < n_live) {
+                        s_mask16[((n_coll + jb) * 4 + l) * 4 + 2 * (wg >> 1)] = (uint16_t)bits[0];
+                        s_mask16[((n_coll + jb) * 4 + l) * 4 + 2 * (wg >> 1) + 1] = (uint16_t)bits[1];
+                    }
                 }
             }
-            if (FUSED && l == nh - 1) {  // output layer (64 -> 2): this thread's 16-column share of both dot products
-                float p0 = 0.f, p1 = 0.f;
+            if (FUSED && l == nh - 1) {  // output layer (64 -> 2): this quad's 32-column share of both dot products
+                float p0[2] = {0.f, 0.f}, p1[2] = {0.f, 0.f};
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    p0 = fmaf(act[j], s_wout[col0 + j], p0);
-                    p1 = fmaf(act[j], s_wout[HID + col0 + j], p1);
+                for (int e = 0; e < 16; ++e) {
+                    const int i = (e >> 1) & 1, c = dc + 8 * (e >> 2) + (e & 1);
+                    p0[i] = fmaf(act[e], s_wout[c], p0[i]);
+                    p1[i] = fmaf(act[e], s_wout[HID + c], p1[i]);
                 }
-                float *s_part = reinterpret_cast<float *>(sL);  // [4 column quarters][128][2]; sL (activation lo) is idle after the last forward MMA
-                s_part[(cq * TM + row) * 2] = p0;
-                s_part[(cq * TM + row) * 2 + 1] = p1;
+                float *s_part = reinterpret_cast<float *>(sL);  // [2 column halves][128][2]; sL (activation lo) is idle after the last forward MMA
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const float s0 = quad_sum(p0[i]), s1 = quad_sum(p1[i]);
+                    if ((lane & 3) == 0) {
+                        s_part[((wg >> 1) * TM + dr + 8 * i) * 2] = s0;
+                        s_part[((wg >> 1) * TM + dr + 8 * i) * 2 + 1] = s1;
+                    }
+                }
             }
-            tc_fence_before();
         }
         if (!ok) break;
+        __syncthreads();  // a_nh (sG) and s_part were written in the fragment layout; steps 2b and 3 read them by row
         if (FUSED) {  // ---- 2b. network outputs -> per-point losses -> cotangent seeds
-            float *s_part = reinterpret_cast<float *>(sL), *s_out = s_part + 4 * TM * 2;
-            __syncthreads();
+            float *s_part = reinterpret_cast<float *>(sL), *s_out = s_part + 2 * TM * 2;
             if (tid < TM) {
-                s_out[2 * tid] = s_part[tid * 2] + s_part[(TM + tid) * 2] + s_part[(2 * TM + tid) * 2] + s_part[(3 * TM + tid) * 2] + s_wout[2 * HID];
-                s_out[2 * tid + 1] = s_part[tid * 2 + 1] + s_part[(TM + tid) * 2 + 1] + s_part[(2 * TM + tid) * 2 + 1] +
-                                     s_part[(3 * TM + tid) * 2 + 1] + s_wout[2 * HID + 1];
+                s_out[2 * tid] = s_part[tid * 2] + s_part[(TM + tid) * 2] + s_wout[2 * HID];
+                s_out[2 * tid + 1] = s_part[tid * 2 + 1] + s_part[(TM + tid) * 2 + 1] + s_wout[2 * HID + 1];
                 s_seed[2 * tid] = 0.f;
                 s_seed[2 * tid + 1] = 0.f;
             }
@@ -838,35 +829,10 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
         }
         // ---- 4. hidden layers, last to first
         for (int l = nh - 1; l >= 0; --l) {
-            fence_proxy_async();
-            __syncthreads();
-            if (tid == 0) {
-                if (l < nh - 1) { ok = mbar_wait_bounded(&s_mbar[1], ph_w); ph_w ^= 1; }
-                tc_fence_after();
-                const uint32_t gB = smem_u32(sG), wB = smem_u32(sW);
-                if (ok) {
-                    if (a.mlp_grad) {  // dW_l^T[k][o] += sum_p a_l[p][k] g_l[p][o]; A = a_l stacked (MN-major), B = g_l (MN-major), K = points
-                        const uint32_t aB = smem_u32(l == 0 ? sF : sAct + (l - 1) * 16 * kGA), ga = l == 0 ? kGA0 : kGA;
-                        uint32_t acc = first_tile ? 0u : 1u;
-                        for (int ks = 0; ks < TM / 16; ++ks) {
-                            const uint64_t ad = make_desc(aB + ks * 2 * ga, ga, 128);
-                            umma_bf16(tmW + 64 * l, ad, make_desc(gB + ks * 2 * kGA, kGA, 128), kIdescAmnBmn, acc); acc = 1;
-                            umma_bf16(tmW + 64 * l, ad, make_desc(gB + 1024 + ks * 2 * kGA, kGA, 128), kIdescAmnBmn, 1);
-                        }
-                    }
-                    // D[p][k] = sum_o g_l[p][o] W_l[o][k]; A = g_l (K-major), B = W_l image (MN-major: N = k, K = o)
-                    uint32_t acc = 0;
-                    for (int ks = 0; ks < HID / 16; ++ks) {
-                        const uint64_t gh = make_desc(gB + ks * 256, 128, kGA), gm = make_desc(gB + 1024 + ks * 256, 128, kGA);
-                        const uint64_t wh = make_desc(wB + ks * 2 * kGW, kGW, 128), wm = make_desc(wB + 1024 + ks * 2 * kGW, kGW, 128);
-                        umma_bf16(tmD, gh, wh, kIdescBmn, acc); acc = 1;
-                        umma_bf16(tmD, gh, wm, kIdescBmn, 1);
-                        umma_bf16(tmD, gm, wh, kIdescBmn, 1);
-                        umma_bf16(tmD, gm, wm, kIdescBmn, 1);
-                    }
-                }
-                umma_commit(&s_mbar[0]);
-            }
+            sync_w(l < nh - 1);
+            if (!ok) break;
+            if (a.mlp_grad) issue_dw(l);  // dW_l^T[k][o] += sum_p a_l[p][k] g_l[p][o]
+            issue_gw();                   // D[p][k] = sum_o g_l[p][o] W_l[o][k]
             if (a.mlp_grad) {  // db_l[o] = sum_p g_l[p][o] while the tensor core works (reads only this thread's own region of sG)
                 float c[16];
                 load8_sum(sG, row, col0, c);
@@ -874,30 +840,20 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
                 const float s = colsum16(c, lane);
                 if (lane < 16) s_col[q * 128 + col0 + lane] = s;
             }
-            ok = mbar_wait_bounded(&s_mbar[0], ph_mma) && ok;
-            ph_mma ^= 1;
-            if (!ok) break;
-            tc_fence_after();
-            if (tid == 0 && l > 0) {
-                mbar_arrive_expect_tx(&s_mbar[1], kWImg);
-                bulk_g2s(sW, wimg + (size_t)(l - 1) * kWImg, kWImg, &s_mbar[1]);
-            }
-            uint32_t v[16];
-            tmem_ld16(tmD + ((uint32_t)(32 * q) << 16) + (uint32_t)col0, v);
+            finish();
+            if (tid == 0 && l > 0) load_w(l - 1);
             if (l > 0) {  // g_{l-1} = D (.) relu'(a_l), in place
-                float m[16], gp[16];
-                load8_hi(sAct + (l - 1) * 16 * kGA, row, col0, m);
-                load8_hi(sAct + (l - 1) * 16 * kGA, row, col0 + 8, m + 8);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) gp[j] = m[j] > 0.f ? __uint_as_float(v[j]) : 0.f;  // a > 0 <=> its bf16 hi part > 0
-                store8(sG, nullptr, row, col0, gp);
-                store8(sG, nullptr, row, col0 + 8, gp + 8);
-            } else if (cq < 2) {  // dL/dfeat in fp32
+                for (int e = 0; e < 16; e += 2) {
+                    const int r = dr + 8 * ((e >> 1) & 1), c = dc + 8 * (e >> 2);
+                    const float2 m = load2_hi(sAct + (l - 1) * 16 * kGA, r, c);  // a > 0 <=> its bf16 hi part > 0
+                    store2(sG, nullptr, r, c, m.x > 0.f ? dD[e] : 0.f, m.y > 0.f ? dD[e + 1] : 0.f);
+                }
+            } else if ((wg >> 1) == 0) {  // dL/dfeat (columns 0..31) in fp32
                 float *gf = reinterpret_cast<float *>(sL);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) gf[row * 33 + col0 + j] = __uint_as_float(v[j]);
+                for (int e = 0; e < 16; ++e) gf[(dr + 8 * ((e >> 1) & 1)) * 33 + dc + 8 * (e >> 2) + (e & 1)] = dD[e];
             }
-            tc_fence_before();
             __syncthreads();
             if (a.mlp_grad && q == 0 && lane < 16) {
                 const int c = col0 + lane;
@@ -952,26 +908,20 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
     }
     if (ANALYTIC && ok && n_coll > 0) second_order();  // the last, partial batch
     __syncthreads();
-    // ---- 6. read the weight-gradient accumulators out of TMEM once
+    // ---- 6. read the weight-gradient accumulators out of the registers once
     if (ok && a.mlp_grad && !first_tile) {
-        tc_fence_after();
         float *G = a.mlp_grad;
-        float *s_stage = reinterpret_cast<float *>(s_tc);  // [128 rows][65] fp32 scratch over the (dead) activation buffers
         for (int l = 0; l < nh; ++l) {
             const int K = l == 0 ? kFeat : HID;
-            uint32_t v[16];
-            tmem_ld16(tmW + 64 * l + ((uint32_t)(32 * q) << 16) + (uint32_t)col0, v);
+            if (wg == l) {  // rows k >= K of the feature layer are the garbage rows of its M = 64 view
 #pragma unroll
-            for (int j = 0; j < 16; ++j) s_stage[row * 65 + col0 + j] = __uint_as_float(v[j]);
-            __syncthreads();
-            // rows k (hi part of a_l[.,k]) and K' + k (mid part), K' = 64 (32 for the feature layer, whose rows 64.. are garbage)
-            for (int e = tid; e < HID * K; e += NT) {
-                const int o = e / K, k = e % K;
-                atomicAdd(G + e, s_stage[k * 65 + o] + s_stage[(K + k) * 65 + o]);
+                for (int e = 0; e < 32; ++e) {
+                    const int k = fr + 8 * ((e >> 1) & 1), o = 8 * (e >> 2) + fc + (e & 1);
+                    if (k < K) atomicAdd(G + (size_t)o * K + k, accW[e]);
+                }
             }
             if (q == 0 && lane < 16) atomicAdd(G + (size_t)HID * K + col0 + lane, dbias[l]);
             G += (size_t)HID * K + HID;
-            __syncthreads();
         }
         if (ANALYTIC && q == 0 && lane < 16) atomicAdd(G + col0 + lane, acc2_wo);  // second-order part of dL/dw_out[0]
         if (tid < HID) atomicAdd(G + tid, dwo0);
@@ -982,11 +932,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
         loss_acc = warp_sum(loss_acc);
         if (lane == 0 && loss_acc != 0.f) atomicAdd(lo.loss_out, loss_acc);
     }
-    __syncthreads();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(512));
-    if (!ok) __trap();
+    if (!ok) __trap();  // the copy engine never signalled: fail loudly rather than return garbage
 }
 
 }  // namespace gssdf
@@ -1001,7 +947,7 @@ extern "C" int64_t gssdf_sdf_mlp_packed_bytes(const gssdf_sdf_net *net) {
 extern "C" int gssdf_sdf_mlp_pack(const gssdf_sdf_net *net, void *packed, gssdf_stream_t stream) {
     GSSDF_REQUIRE(net && packed, GSSDF_EINVAL, "sdf_mlp_pack: null argument");
     GSSDF_REQUIRE(net->hidden_dim == 64 && net->n_levels * net->n_features_per_level == kFeat, GSSDF_EUNSUPPORTED,
-                  "sdf_mlp_pack: the tcgen05 decoder needs hidden_dim 64 and 32 encoded features");
+                  "sdf_mlp_pack: the tensor-core decoder needs hidden_dim 64 and 32 encoded features");
     GSSDF_REQUIRE(net->n_hidden >= 0 && net->n_hidden <= 3, GSSDF_EUNSUPPORTED, "sdf_mlp_pack: n_hidden %d not in [0,3]", net->n_hidden);
     GSSDF_REQUIRE(net->mlp, GSSDF_EINVAL, "sdf_mlp_pack: net.mlp is null");
     GSSDF_REQUIRE(((uintptr_t)packed & 15) == 0, GSSDF_EINVAL, "sdf_mlp_pack: packed must be 16-byte aligned");
@@ -1011,8 +957,8 @@ extern "C" int gssdf_sdf_mlp_pack(const gssdf_sdf_net *net, void *packed, gssdf_
 }
 
 static int check_tc(const char *who, const gssdf_sdf_net &net) {
-    GSSDF_REQUIRE(net.hidden_dim == 64, GSSDF_EUNSUPPORTED, "%s: the tcgen05 decoder needs hidden_dim 64", who);
-    GSSDF_REQUIRE(net.n_hidden <= 3, GSSDF_EUNSUPPORTED, "%s: the tcgen05 decoder supports n_hidden <= 3 (TMEM holds 4 weight-gradient tiles)", who);
+    GSSDF_REQUIRE(net.hidden_dim == 64, GSSDF_EUNSUPPORTED, "%s: the tensor-core decoder needs hidden_dim 64", who);
+    GSSDF_REQUIRE(net.n_hidden <= 3, GSSDF_EUNSUPPORTED, "%s: the tensor-core decoder supports n_hidden <= 3 (one weight-gradient accumulator per warpgroup)", who);
     GSSDF_REQUIRE(net.mlp_packed && ((uintptr_t)net.mlp_packed & 15) == 0, GSSDF_EINVAL,
                   "%s: mlp_mode 1 needs net.mlp_packed (gssdf_sdf_mlp_pack), 16-byte aligned", who);
     return GSSDF_OK;
@@ -1021,14 +967,14 @@ static int check_tc(const char *who, const gssdf_sdf_net &net) {
 extern "C" int gssdf_sdf_fwd_tc_launch(const gssdf_sdf_fwd_args *a, const gssdf::GridGeom *g, gssdf_stream_t stream) {
     int rc = check_tc("sdf_fwd", a->net);
     if (rc) return rc;
-    const size_t smem = 16 * kGA + 16 * kGA0 + 16 * kGL + kWImg + sizeof(float) * (5 * 64 + 132 + 2 * 128 * 2) + 1024;
+    const size_t smem = 16 * kGA + 16 * kGA0 + 16 * kGL + kWImg + sizeof(float) * (5 * 64 + 132) + 1024;
     static bool attr_set = false;
     if (!attr_set) {
         GSSDF_CUDA_OK(cudaFuncSetAttribute(sdf_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     const int64_t n_tiles = (a->n * (a->n_variants > 1 ? a->n_variants : 1) + 127) / 128;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)2 * sms);  // two ~90 KiB CTAs fit one SM
@@ -1042,7 +988,7 @@ extern "C" int gssdf_sdf_bwd_tc_launch(const gssdf_sdf_bwd_args *a, const gssdf:
     if (rc) return rc;
     GSSDF_CUDA_OK(cudaFuncSetAttribute(sdf_bwd_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_tc_smem(false)));
     const int64_t n_tiles = (a->n * (a->n_variants > 1 ? a->n_variants : 1) + 127) / 128;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms);
@@ -1080,7 +1026,7 @@ extern "C" int gssdf_sdf_train(const gssdf_sdf_train_args *t, gssdf_stream_t str
     GSSDF_CUDA_OK(cudaFuncSetAttribute(sdf_bwd_tc_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_tc_smem(true)));
     const int pt = 128 / t->n_variants;
     const int64_t n_tiles = (t->n + pt - 1) / pt;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms);

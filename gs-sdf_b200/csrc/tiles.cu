@@ -7,7 +7,7 @@
 // packed-index order, radix-sorts all n_isects pairs over 42-48 key bits (6 global passes) and
 // derives per-tile offsets from the sorted keys, with two host syncs in between.
 //
-// B200-first method (same bits out, ~8x less HBM traffic, no host sync):
+// Method (same bits out, ~8x less HBM traffic, no host sync):
 //   1. tile_count   : per splat tile rect -> tiles_per_gauss + per-(camera,tile) histogram
 //   2. scan         : exclusive scan of the histogram == isect_offsets, total == n_isects
 //   3. tile_scatter : every intersection is written into its tile's bin as the unique 64-bit key
@@ -421,7 +421,7 @@ extern "C" int gssdf_tile_encode(const gssdf_tile_encode_args *a, gssdf_stream_t
     ws += align_up((size_t)(a->isect_cap > 0 ? a->isect_cap : 1) * 8, 256);
     int32_t *big = reinterpret_cast<int32_t *>(ws);
     constexpr int SS = 256, S0 = 2048, S1 = 8192, S2 = 28672;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 

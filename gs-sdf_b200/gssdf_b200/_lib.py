@@ -85,7 +85,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(SO_PATH):
             raise RuntimeError(
-                f"{SO_PATH} not found: build it with `python gs-sdf_b200/build.py` (nvcc, sm_100a). "
+                f"{SO_PATH} not found: build it with `python gs-sdf_b200/build.py` (nvcc, sm_90a). "
                 "gssdf_b200 has no CPU/PyTorch fallback.")
         L = C.CDLL(SO_PATH)
         for name, (ret, _args) in FUNCS.items():

@@ -8,7 +8,7 @@ Same names, argument meaning, return arity and error behaviour as the reference'
                                 GSC/isect_tiles.hpp:8-46, GSC/rendering.h:15-20 (.cpp:49-63)
   rasterize_to_pixels_2dgs      GSC/rasterize_to_pixels.h:64-80    (.cpp:170-381)
   rasterization_2dgs_sdf        include/neural_gaussian/neural_gaussian.cpp:129-271
-All compute happens in libgssdf_b200.so (hand-written sm_100a CUDA) through gssdf_b200.cabi; torch is
+All compute happens in libgssdf_b200.so (hand-written sm_90a CUDA) through gssdf_b200.cabi; torch is
 used for device memory, streams and autograd plumbing only. The C++/libtorch twin of this file, meant
 to be linked into neural_mapping_node, is gs-sdf_b200/shim/.
 

@@ -125,9 +125,8 @@ class SparseRowExchange:
         self.cnt_ev.synchronize()
         rows = (int(self.cnt_host.max()) + 255) // 256 * 256
         self.rows = min(max(rows, 256), self._N)
-        # measured on B200 / NVLink 5 (profiles/r2y_*.json): at 2 ranks (gathered rows = 0.31 x the dense segment) the rows win (4.68 vs
-        # 4.77 ms / step); at 4 ranks (0.62 x) the shorter wait is eaten by the pack / unpack launches and the host read of the counts
-        # (5.09 vs 5.05 ms): sparse only while the gathered rows are clearly smaller
+        # the row exchange saves wire time but adds pack / unpack launches and a host read of the counts: sparse only while the
+        # gathered rows are clearly smaller than the dense segment
         return self.always or self.world * self.rows * self.stride * 4 <= 0.5 * self.dense_bytes
 
     def launch(self):

@@ -66,7 +66,7 @@ class SdfNet(torch.nn.Module):
         assert self.decoder_.numel() == n_mlp
         self._half = torch.empty(n_table, dtype=torch.float16, device=device)
         self._half_version = None
-        # decoder arithmetic: tcgen05 tensor cores where supported (hidden 64, <= 3 hidden->hidden layers), else fp32 CUDA cores
+        # decoder arithmetic: wgmma tensor cores where supported (hidden 64, <= 3 hidden->hidden layers), else fp32 CUDA cores
         self.mlp_mode = (1 if hidden_dim == 64 and geo_num_layer <= 3 else 0) if mlp_mode is None else int(mlp_mode)
         self._packed = torch.empty(cabi.sdf_mlp_packed_bytes(probe), dtype=torch.uint8, device=device) if self.mlp_mode == 1 else None
         self._packed_version = None

@@ -1,5 +1,5 @@
 /*
- * gssdf_b200 -- C ABI of the B200-native GS-SDF hot path (libgssdf_b200.so).
+ * gssdf_b200 -- C ABI of the H100-native GS-SDF hot path (libgssdf_b200.so).
  *
  * Every entry point replaces one host function of the reference's gsplat fork / tcnn binding
  * (the functions the reference's libtorch wrappers `gsplat_cpp` and `tcnn_binding` call) and is
@@ -46,7 +46,7 @@ enum {
 };
 
 const char *gssdf_last_error(void);
-/* "gssdf_b200 <ver> sm_100a" */
+/* "gssdf_b200 <ver> sm_90a" */
 const char *gssdf_version(void);
 /* Argument structs grow between revisions: a binding compiled against this header must see the same number from the library. */
 #define GSSDF_ABI_REVISION 14
@@ -199,7 +199,7 @@ int gssdf_view_colors_bwd(const gssdf_view_colors_bwd_args *a, gssdf_stream_t st
  *       isect_ids[i]  = cid << (32+tile_n_bits) | tile_id << 32 | float_bits(depth)  (sorted)
  *       flatten_ids[i]= packed splat index, ties in emission order
  *       offsets[c,ty,tx] = first i of that tile (== n_isects for trailing empty tiles)
- *     Method (B200-first, no 6-pass global radix sort): per-tile histogram -> scan (= offsets) ->
+ *     Method (no 6-pass global radix sort): per-tile histogram -> scan (= offsets) ->
  *     binned scatter -> per-tile shared-memory sort of the unique key (depth_bits, packed index).
  * ------------------------------------------------------------------------------------------ */
 typedef struct gssdf_tile_encode_args {
@@ -410,8 +410,8 @@ typedef struct gssdf_sdf_net {
     float inv_size;         /*   include/neural_net/sub_map.cpp:82-97); inv_size == 0 -> x is already in [0,1]^3 */
     int32_t mlp_mode;       /* decoder arithmetic (forward and backward):
                                0 = fp32 FMA on the CUDA cores;
-                               1 = 5th-gen tensor cores (hidden_dim 64 only): tcgen05.mma kind::f16 on bf16 splits of both operands
-                                   with fp32 accumulation in TMEM. Forward / forward-recompute: 3-term split (24 significant bits,
+                               1 = Hopper tensor cores (hidden_dim 64 only): wgmma.mma_async on bf16 splits of both operands
+                                   with fp32 accumulation in registers. Forward / forward-recompute: 3-term split (24 significant bits,
                                    6 products -> fp32-grade pre-activations, so ReLU decisions match the fp32 path); backward
                                    GEMMs: 2-term split, 4 products (~2^-17 relative). Needs mlp_packed. */
     const void *mlp_packed; /* mode 1 only: [gssdf_sdf_mlp_packed_bytes] the hidden layers' weights pre-split into bf16 hi/mid/lo in

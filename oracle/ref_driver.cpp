@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY. Thin pybind11 driver around the UNMODIFIED kernel launchers of the reference's
 // gsplat fork, compiled from where they lie under /root/reference by oracle/build_ref.py into
-// oracle/_ref/gsplat_ref*.so. It exists to run the reference CUDA kernels on the B200 box and dump golden
+// oracle/_ref/gsplat_ref*.so. It exists to run the reference CUDA kernels on a GPU and dump golden
 // vectors (oracle/gen_golden_ref.py). The host glue below (two-pass compaction, cumsum, output
 // allocation) is written against the launcher declarations in GSF/csrc/{Projection,Intersect,
 // Rasterization,SphericalHarmonics}.h and follows the call order of GSF/csrc/Projection.cpp:654-774,

@@ -17,7 +17,7 @@
  * Pinning: tiny-cuda-nn ships no tests and GS-SDF none (SURVEY 4), and tcnn's runtime was not built here (its own cmake, minutes per
  * TU). The grid KERNELS, however, are header templates: oracle/ref_tcnn_grid_driver.cu instantiates the reference's kernel_grid,
  * kernel_grid_backward, kernel_grid_backward_input, kernel_grid_backward_input_backward_grid/_dLdoutput directly from grid.h; they were
- * run on a B200 (oracle/gen_golden_tcnn.py -> tests/golden/tcnn_grid_ref.npz) and this file reproduces their outputs: encoded features
+ * run on an H100 (oracle/gen_golden_tcnn.py -> tests/golden/tcnn_grid_ref.npz) and this file reproduces their outputs: encoded features
  * bit-for-bit, dy_dx / dL/dx to fp32 rounding, table gradients to the accuracy of the reference's half atomics
  * (tests/test_sdf_oracle.py::test_oracle_grid_matches_tiny_cuda_nn_kernels). The decoder (libtorch Linear/ReLU) and the
  * second-order chains are pinned against torch.autograd (same file).

@@ -19,7 +19,7 @@
  *     implementations (gsplat/cuda/_torch_impl.py::_isect_tiles/_isect_offset_encode/
  *     _spherical_harmonics, the checkers of GSR/tests/test_basic.py::test_isect/test_sh),
  *   - tests/golden/ref_cuda_*.npz: outputs of the reference's CUDA kernels compiled from
- *     /root/reference (oracle/build_ref.py) and run on a B200 (oracle/gen_golden_ref.py).
+ *     the reference sources (oracle/build_ref.py) and run on an H100 (oracle/gen_golden_ref.py).
  */
 #include <math.h>
 #include <stdint.h>

@@ -1,6 +1,6 @@
 """Checks shared by the CPU test (oracle vs reference-CUDA goldens) and the GPU test (our kernels vs the same
 goldens). A golden file holds every tensor of one call chain of rasterization_2dgs_sdf produced by the reference
-fork's own CUDA kernels on a B200 (oracle/gen_golden_ref.py)."""
+fork's own CUDA kernels on an H100 (oracle/gen_golden_ref.py)."""
 import numpy as np
 
 from helpers import assert_close_frac

@@ -122,7 +122,7 @@ def test_hashgrid_operators_vs_oracle(oracle, log2):
 @pytest.mark.parametrize("name", ["tcnn_grid_ref.npz", "tcnn_grid_ref19.npz"])
 def test_hashgrid_operators_vs_tiny_cuda_nn_goldens(name):
     """Our operator-level kernels fed with the SAME inputs as tiny-cuda-nn's own kernels (goldens from oracle/gen_golden_tcnn.py run on a
-    B200): kernel_grid, kernel_grid_backward(+_input), kernel_grid_backward_input_backward_{grid,dLdoutput,input}."""
+    H100): kernel_grid, kernel_grid_backward(+_input), kernel_grid_backward_input_backward_{grid,dLdoutput,input}."""
     from gssdf_b200 import cabi
     path = os.path.join(HERE, "golden", name)
     if not os.path.exists(path):
@@ -439,7 +439,7 @@ def test_coupling_site_sample_gate(oracle, mode):
     la, tga, mga, vxa = run(_t(x, dev), _t(w, dev), _t(vis, dev), True)
     lb, tgb, mgb, vxb = run(_t(x[sel], dev), _t(w[sel], dev), _t(vis[sel], dev), False)
     assert abs(la - lb) <= 1e-5 * abs(lb) and lb != 0.0
-    # (same arithmetic per point; the points sit in different tiles, so the fp32 / TMEM accumulation order of the sums differs)
+    # (same arithmetic per point; the points sit in different tiles, so the fp32 accumulation order of the sums differs)
     assert rel(mga, mgb) <= 1e-4 and rel(tga, tgb) <= 1e-4
     assert np.abs(vxa[~sel]).max() == 0.0 and rel(vxa[sel], vxb) <= 1e-4
     if mode == "numerical":  # the three-call path (sdf_loss) applies the same gate

@@ -171,7 +171,7 @@ def _tc_net(cabi, half, mlp_t, n_hidden):
 
 @pytest.mark.parametrize("n,n_hidden,variants", [(5000, 3, 1), (1000, 1, 7), (130, 0, 1)])
 def test_sdf_fwd_tensor_core_path(oracle, n, n_hidden, variants):
-    """mlp_mode=1: decoder on the 5th-gen tensor cores (tcgen05.mma, bf16 hi/mid split, fp32 accumulate in TMEM).
+    """mlp_mode=1: decoder on the Hopper tensor cores (wgmma, bf16 hi/mid split, fp32 accumulate in registers).
     Features stay bit-exact; sdf/y1 within 1e-4 relative (+1e-5 absolute, the same bar as the fp32 CUDA-core path) of the fp64
     oracle: the forward uses a 3-term bf16 split of both operands (24 significant bits)."""
     from gssdf_b200 import cabi
@@ -193,14 +193,14 @@ def test_sdf_fwd_tensor_core_path(oracle, n, n_hidden, variants):
     pts = (x[None] + offs[:, None]).reshape(-1, 3).astype(np.float32)
     r_sdf, r_y1, r_feat = oracle.sdf_fwd(pts, table, mlp, 64, n_hidden)
     assert np.array_equal(feat.cpu().numpy(), r_feat)
-    assert_close_frac(sdf.cpu().numpy(), r_sdf, 1e-4, 1e-5, 0.0, "sdf (tcgen05)")
-    assert_close_frac(y1.cpu().numpy(), r_y1, 1e-4, 1e-5, 0.0, "y1 (tcgen05)")
+    assert_close_frac(sdf.cpu().numpy(), r_sdf, 1e-4, 1e-5, 0.0, "sdf (tensor cores)")
+    assert_close_frac(y1.cpu().numpy(), r_y1, 1e-4, 1e-5, 0.0, "y1 (tensor cores)")
 
 
 @pytest.mark.parametrize("n,n_hidden,variants", [(5000, 3, 1), (40000, 3, 1), (1000, 1, 7), (130, 0, 1)])
 def test_sdf_bwd_tensor_core_path(oracle, n, n_hidden, variants):
-    """mlp_mode=1 backward: forward recompute, dL/da GEMMs and the weight-gradient GEMMs (accumulated in TMEM across the
-    persistent CTA's tiles) all on tcgen05; compared with the fp64 oracle chain at the same tolerances as the SIMT path
+    """mlp_mode=1 backward: forward recompute, dL/da GEMMs and the weight-gradient GEMMs (accumulated in registers across the
+    persistent CTA's tiles) all on wgmma; compared with the fp64 oracle chain at the same tolerances as the SIMT path
     (a slightly larger absolute floor for the 16-bit operand split)."""
     from gssdf_b200 import cabi
     dev = _dev()
@@ -225,11 +225,11 @@ def test_sdf_bwd_tensor_core_path(oracle, n, n_hidden, variants):
     torch.cuda.synchronize()
     r_tg, r_mg, r_vx = oracle.sdf_bwd(pts, table, mlp, v_sdf, v_y1, 64, n_hidden)
     mgc, tgc, vxc = mg.cpu().numpy(), tg.cpu().numpy(), vx.cpu().numpy()
-    assert_close_frac(mgc, r_mg, 1e-4, 3e-5 * np.abs(r_mg).max(), 0.0, "mlp grad (tcgen05)")
+    assert_close_frac(mgc, r_mg, 1e-4, 3e-5 * np.abs(r_mg).max(), 0.0, "mlp grad (tensor cores)")
     assert np.linalg.norm(mgc - r_mg) <= 5e-5 * np.linalg.norm(r_mg)
-    assert_close_frac(tgc, r_tg, 2e-3, 1e-5 * np.abs(r_tg).max(), 1e-3, "table grad (tcgen05)")
+    assert_close_frac(tgc, r_tg, 2e-3, 1e-5 * np.abs(r_tg).max(), 1e-3, "table grad (tensor cores)")
     assert np.linalg.norm(tgc - r_tg) <= 2e-4 * np.linalg.norm(r_tg)
-    assert_close_frac(vxc, r_vx[:n], 2e-3, 1e-4 * np.abs(r_vx).max(), 1e-3, "v_x (tcgen05)")
+    assert_close_frac(vxc, r_vx[:n], 2e-3, 1e-4 * np.abs(r_vx).max(), 1e-3, "v_x (tensor cores)")
     assert np.linalg.norm(vxc - r_vx[:n]) <= 5e-4 * np.linalg.norm(r_vx[:n])
 
 
@@ -284,7 +284,7 @@ def test_sdf_train_fused_equals_separate_calls(oracle, case):
 
 
 def test_full_step_tensor_core_equals_cuda_core_path():
-    """GsSdfStep ([A] SDF on rays, [B] render, [C] GS<->SDF coupling, [D] backward) with the fused tcgen05 SDF kernels (mlp_mode 1)
+    """GsSdfStep ([A] SDF on rays, [B] render, [C] GS<->SDF coupling, [D] backward) with the fused tensor-core SDF kernels (mlp_mode 1)
     vs the three-call fp32 CUDA-core path (mlp_mode 0): losses and every segment of the flat gradient agree."""
     import math
     from gssdf_b200 import render, scene as S
@@ -444,7 +444,7 @@ def test_sdf_train_small_and_ragged_batches(oracle, n, live):
 
 
 def test_cuda_features_match_tiny_cuda_nn_kernels(oracle):
-    """The CUDA encoder against the outputs of tiny-cuda-nn's own kernel_grid run on a B200 (tests/golden/tcnn_grid_ref.npz; level 0
+    """The CUDA encoder against the outputs of tiny-cuda-nn's own kernel_grid run on an H100 (tests/golden/tcnn_grid_ref.npz; level 0
     dense incl. cube-face points, levels 1-15 hashed at log2_hashmap_size 16): bit-identical features, both arithmetic modes."""
     import os
     from gssdf_b200 import cabi

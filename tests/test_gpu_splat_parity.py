@@ -366,7 +366,7 @@ def test_error_conventions():
 
 def test_kernels_vs_reference_cuda_goldens(oracle):
     """Our CUDA kernels fed with the reference fork's own tensors (tests/golden/ref_cuda_*.npz, produced by the
-    reference kernels on a B200) reproduce the reference's outputs: ints bit-exact, floats to 1e-4-ish
+    reference kernels on an H100) reproduce the reference's outputs: ints bit-exact, floats to 1e-4-ish
     (both sides are fast-math fp32), gradients within the reference's own run-to-run spread."""
     import glob
     import os

@@ -171,7 +171,7 @@ def _tcnn_golden():
 def test_oracle_grid_matches_tiny_cuda_nn_kernels(oracle):
     """The hash-grid restatement against outputs of tiny-cuda-nn's OWN kernels (kernel_grid, kernel_grid_backward,
     kernel_grid_backward_input, kernel_grid_backward_input_backward_grid/_dLdoutput from the reference's grid.h, instantiated by
-    oracle/ref_tcnn_grid_driver.cu and run on a B200: tests/golden/tcnn_grid_ref.npz, generator oracle/gen_golden_tcnn.py)."""
+    oracle/ref_tcnn_grid_driver.cu and run on an H100: tests/golden/tcnn_grid_ref.npz, generator oracle/gen_golden_tcnn.py)."""
     g, table, cfg = _tcnn_golden()
     x, n_params = g["x"], int(g["n_params"])
     assert oracle.grid_setup(**{k: cfg[k] for k in ("L", "F", "log2_hashmap", "base_res", "per_level_scale")})[0] == n_params

@@ -1,4 +1,4 @@
-"""Condense an ncu --set full report (.ncu-rep) into the handful of metrics quoted in profiles/*.md and DESIGN.md."""
+"""Condense an ncu --set full report (.ncu-rep) into a handful of per-kernel metrics."""
 import csv
 import io
 import subprocess
