@@ -11,6 +11,8 @@
   local_map_checkpoint.pt torch::save(local_map_ptr) (neural_mapping.cpp:1331-1342): a libtorch module archive with the flat tcnn parameter
                           `encoder_local_map` and `decoder.{0,2,4,..}.{weight,bias}`; written / read through the libtorch shim
                           (gssdf_shim.LocalMapReplay.save / .load), because only libtorch can produce its own archive format.
+  mesh_*.ply              NeuralSLAM::save_mesh -> mc::save_mesh_as_ply (include/mesher/cumcubes/src/cumcubes.cpp:30-80): binary PLY with
+                          float x y z + uchar red green blue per vertex and `list int int vertex_index` triangles
 Host-side file I/O only: numpy + torch tensors, no device code."""
 import math
 import os
@@ -133,3 +135,45 @@ def read_pt_params(path, leaf_size):
     res = 2 ** level
     return dict(map_origin=origin, inner_map_size=inner, package_path=pkg.group(1).strip() if pkg else "", x_max=0.5 * inner, x_min=-0.5 * inner,
                 octree_level=level, map_resolution=res, map_size=res * leaf_size, map_size_inv=1.0 / (res * leaf_size))
+
+
+def save_mesh_as_ply(path, vertices, faces, colors):
+    """mc::save_mesh_as_ply (include/mesher/cumcubes/src/cumcubes.cpp:30-80): binary little-endian PLY; per vertex `float x y z` +
+    `uchar red green blue` (15 bytes, unpadded), per face `property list int int vertex_index` (the count 3 as int32, then three int32).
+    vertices [V,3] float32, faces [F,3] int32, colors [V,3] uint8 (torch tensors on any device, or numpy arrays)."""
+    c = lambda t: t.detach().cpu().numpy() if hasattr(t, "detach") else np.asarray(t)
+    v, f, col = c(vertices).astype("<f4").reshape(-1, 3), c(faces).astype("<i4").reshape(-1, 3), c(colors).astype("u1").reshape(-1, 3)
+    if len(col) != len(v):
+        raise ValueError(f"save_mesh_as_ply: {len(v)} vertices but {len(col)} colours")
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}", "property float x", "property float y", "property float z",
+            "property uchar red", "property uchar green", "property uchar blue", f"element face {len(f)}",
+            "property list int int vertex_index", "end_header"]
+    rec = np.empty(len(v), np.dtype([("xyz", "<f4", 3), ("rgb", "u1", 3)]))
+    rec["xyz"], rec["rgb"] = v, col
+    fr = np.empty((len(f), 4), "<i4")
+    fr[:, 0], fr[:, 1:] = 3, f
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(head) + "\n").encode("ascii"))
+        fh.write(rec.tobytes())
+        fh.write(fr.tobytes())
+
+
+def read_mesh_ply(path):
+    """Reads what save_mesh_as_ply (or the reference's writer) wrote: (vertices [V,3] float32, faces [F,3] int32, colors [V,3] uint8) as
+    numpy arrays. Only that layout is accepted: triangles, `list int int`, x y z float + red green blue uchar."""
+    with open(path, "rb") as fh:
+        raw = fh.read()
+    end = raw.index(b"end_header\n") + len(b"end_header\n")
+    head = raw[:end].decode("ascii").splitlines()
+    m_v = re.search(r"element vertex (\d+)", "\n".join(head))
+    m_f = re.search(r"element face (\d+)", "\n".join(head))
+    want = ["property float x", "property float y", "property float z", "property uchar red", "property uchar green",
+            "property uchar blue", "property list int int vertex_index"]
+    if head[:2] != ["ply", "format binary_little_endian 1.0"] or not m_v or not m_f or [h for h in head if h.startswith("property")] != want:
+        raise ValueError(f"{path}: not a mesh PLY in the layout of mc::save_mesh_as_ply")
+    nv, nf = int(m_v.group(1)), int(m_f.group(1))
+    rec = np.frombuffer(raw, np.dtype([("xyz", "<f4", 3), ("rgb", "u1", 3)]), count=nv, offset=end)
+    fr = np.frombuffer(raw, "<i4", count=4 * nf, offset=end + 15 * nv).reshape(nf, 4)
+    if nf and not (fr[:, 0] == 3).all():
+        raise ValueError(f"{path}: only triangle faces are supported")
+    return rec["xyz"].astype(np.float32), fr[:, 1:].astype(np.int32), rec["rgb"].astype(np.uint8)

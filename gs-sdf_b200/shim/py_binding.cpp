@@ -5,11 +5,14 @@
 #include "gsplat_cpp/fully_fused_projection.h"
 #include "gsplat_cpp/rasterize_to_pixels.h"
 #include "gsplat_cpp/rendering.h"
+#include "cumcubes.hpp"
 
 void bind_tcnn(pybind11::module &m);
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     bind_tcnn(m);
+    m.def("mc_marching_cubes", &mc::marching_cubes);
+    m.def("mc_save_mesh_as_ply", &mc::save_mesh_as_ply);
     m.def("fully_fused_projection_2dgs", &fully_fused_projection_2dgs);
     m.def("get_view_colors", [](const torch::Tensor &viewmats, const torch::Tensor &means, const torch::Tensor &radii,
                                 const torch::Tensor &colors, const torch::Tensor &camera_ids, const torch::Tensor &gaussian_ids,

@@ -49,7 +49,7 @@ const char *gssdf_last_error(void);
 /* "gssdf_b200 <ver> sm_90a" */
 const char *gssdf_version(void);
 /* Argument structs grow between revisions: a binding compiled against this header must see the same number from the library. */
-#define GSSDF_ABI_REVISION 14
+#define GSSDF_ABI_REVISION 15
 int32_t gssdf_abi_revision(void);
 
 /* L2 residency hint (SURVEY 7.6): marks [ptr, ptr+bytes) as a persisting access-policy window for kernels launched on `stream` from now on
@@ -862,6 +862,33 @@ typedef struct gssdf_sdf_sample_rays_args {
 } gssdf_sdf_sample_rays_args;
 size_t gssdf_sdf_sample_rays_workspace_bytes(int64_t n_rays, int64_t nugget_cap, int32_t voxel_sample_num, int32_t n_free, int32_t n_surface);
 int gssdf_sdf_sample_rays(const gssdf_sdf_sample_rays_args *a, gssdf_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * f-5  Marching cubes over a dense fp32 field.  Replaces mc::marching_cubes (include/mesher/cumcubes/src/cumcubes.cpp:9-28, kernels
+ *     cumcubes_kernel.cu:7-282).  "Inside" is value > thresh. One vertex per crossing lattice edge at
+ *     lower + (i + dt) * scale, dt = (thresh - a) / (b - a), scale = (upper - lower) / n, rounded exactly as the reference's kernel and
+ *     its two ATen ops round them (bit-identical positions). Triangles come from the case table generated by
+ *     gs-sdf_b200/tools/gen_mc_table.py, oriented with their normal toward increasing value.
+ *     Count -> scan -> emit with device-side counts, no host sync, no atomics: vertices are in lattice-edge order (x, y, z, axis),
+ *     faces in cell order then table order -- the same output on every run (the reference's order depends on atomic arrival).
+ *     Writes stop at the capacities; counts[2] then flags the overflow (bit 0 vertices, bit 1 faces) and the true counts are still
+ *     reported, so the caller can grow its buffers and call again.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct gssdf_marching_cubes_args {
+    int32_t nx, ny, nz;           /* lattice size; counts are int32, so 3 * nx*ny*nz and 5 * (nx-1)(ny-1)(nz-1) must stay below 2^31
+                                     (GSSDF_EINVAL otherwise) */
+    const float *grid;            /* [nx,ny,nz] x-major (grid[(x*ny + y)*nz + z]) */
+    float thresh;
+    float lower[3], upper[3];
+    int64_t vertex_cap, face_cap; /* rows allocated in vertices / faces */
+    float *vertices;              /* [vertex_cap,3] */
+    int32_t *faces;               /* [face_cap,3] vertex ids */
+    int32_t *counts;              /* device int32[4], overwritten: n_vertices, n_faces, overflow flags, 0 */
+    void *workspace;              /* >= gssdf_marching_cubes_workspace_bytes(nx, ny, nz) */
+    size_t workspace_bytes;
+} gssdf_marching_cubes_args;
+size_t gssdf_marching_cubes_workspace_bytes(int32_t nx, int32_t ny, int32_t nz);
+int gssdf_marching_cubes(const gssdf_marching_cubes_args *a, gssdf_stream_t stream);
 
 #ifdef __cplusplus
 }
