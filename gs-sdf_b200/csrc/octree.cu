@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "octree_query.cuh"
 
 namespace gssdf {
 
@@ -27,43 +28,13 @@ __constant__ uint8_t c_voxel_order[8][8] = {{0, 1, 2, 4, 3, 5, 6, 7}, {1, 0, 3, 
 
 constexpr int kMaxOctLevel = 15;  // KAOLIN_SPC_MAX_LEVELS
 
-__device__ __forceinline__ void to_m1p1(const gssdf_octree &t, const float *x, float out[3]) {
-#pragma unroll
-    for (int d = 0; d < 3; ++d)  // scale_to_m1p1(_xyz - pos) = (x - pos) * 2 * k_map_size_inv, each op rounded (ATen ops)
-        out[d] = t.inv_size != 0.f ? __fmul_rn(__fmul_rn(__fsub_rn(x[d], t.origin[d]), 2.f), t.inv_size) : x[d];
-}
-
-// identify (KA/spc_utils.cuh:28-61)
-__device__ __forceinline__ int32_t identify(int kx, int ky, int kz, int level, const int32_t *__restrict__ exsum, const uint8_t *__restrict__ octree) {
-    const int maxval = (1 << level) - 1;
-    if (kx < 0 || ky < 0 || kz < 0 || kx > maxval || ky > maxval || kz > maxval) return -1;
-    int ord = 0;
-    for (int l = 0; l < level; ++l) {
-        const int depth = level - l - 1;
-        const unsigned child = (((unsigned)kx >> depth) & 1u) << 2 | (((unsigned)ky >> depth) & 1u) << 1 | (((unsigned)kz >> depth) & 1u);
-        const unsigned bits = __ldg(octree + ord);
-        if (!(bits & (1u << child))) return -1;
-        ord = __ldg(exsum + ord) + __popc(bits & ((2u << child) - 1u));
-    }
-    return ord;
-}
-
 __global__ void __launch_bounds__(256) octree_query_kernel(const gssdf_octree_query_args a) {
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
     const int64_t nl = a.n_live ? min((int64_t)*a.n_live, a.n) : a.n;
     if (i >= nl) return;
-    float c[3];
     const float x[3] = {__ldg(a.coords + 3 * i), __ldg(a.coords + 3 * i + 1), __ldg(a.coords + 3 * i + 2)};
-    to_m1p1(a.tree, x, c);
-    const float res = 0.5f * exp2f((float)a.tree.level);  // query_cuda_kernel: floor(resolution * (c + 1)) -> short (saturating)
     int k[3];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-        const float v = floorf(__fmul_rn(res, __fadd_rn(c[d], 1.0f)));
-        k[d] = (int)fminf(fmaxf(v, -32768.f), 32767.f);
-        if (!(v == v)) k[d] = 0;  // NaN -> 0 like cvt.rzi.s16.f32
-    }
-    const int32_t p = identify(k[0], k[1], k[2], a.tree.level, a.tree.exsum, a.tree.octree);
+    const int32_t p = query_leaf(a.tree, x, k);
     if (a.pidx) a.pidx[i] = p;
     if (a.valid) a.valid[i] = p > -1 ? 1 : 0;
 }

@@ -89,3 +89,76 @@ CONFIGS = {
     "c4": dict(W=1920, H=1080, N=1_000_000, sh_degree=3),  # per scene / per GPU
     "c5": dict(W=3840, H=2160, N=5_000_000, sh_degree=3),
 }
+
+
+def box_signed_distance(x):
+    """Signed distance to the walls of the BOX room, positive inside (free space), float64 numpy or torch [n,3]."""
+    if hasattr(x, "detach"):
+        import torch
+        b = torch.as_tensor(BOX, dtype=x.dtype, device=x.device)
+        q = x.abs() - b
+        outside = q.clamp_min(0).norm(dim=-1)
+        inside = q.max(-1).values.clamp_max(0)
+        return -(outside + inside)
+    q = np.abs(x) - BOX
+    return -(np.linalg.norm(np.maximum(q, 0), axis=-1) + np.minimum(q.max(-1), 0))
+
+
+def box_wall_points(spacing, offsets=(0.0,)):
+    """Regular samples of the six inside faces of the BOX room, shifted along the wall normal by each of `offsets` (float32 [n,3])."""
+    out = []
+    for a in range(3):
+        o = [i for i in range(3) if i != a]
+        u = np.arange(-BOX[o[0]], BOX[o[0]] + 1e-9, spacing)
+        v = np.arange(-BOX[o[1]], BOX[o[1]] + 1e-9, spacing)
+        uu, vv = np.meshgrid(u, v, indexing="ij")
+        for sgn in (-1.0, 1.0):
+            for off in offsets:
+                p = np.zeros((uu.size, 3))
+                p[:, a] = sgn * (BOX[a] + off)
+                p[:, o[0]], p[:, o[1]] = uu.reshape(-1), vv.reshape(-1)
+                out.append(p)
+    return np.ascontiguousarray(np.concatenate(out), np.float32)
+
+
+def box_room_sdf_net(device, inner_map_size=14.0, leaf_size=0.05, steps=1000, seed=0, pos_W_M=(0.0, 0.0, 0.0), mlp_mode=None, batch=1 << 16):
+    """A SubMap holding the BOX room: (SdfNet, OctreeAS, (xyz_min_M_margin, xyz_max_M_margin)).
+    Octree as SubMap::update_octree_as (sub_map.cpp:22-35): quantise, unique, 27-neighbour dilation, clamp; applied to points on the walls
+    and up to one leaf to either side of them, so that the walls lie well inside the dilated octree. Level and map size as params.cpp:474-478.
+    The net is fitted with the autograd mirror (sdf.SdfNet) and torch.optim.Adam to the room's signed distance, positive inside.
+    Test and benchmark infrastructure (GPU)."""
+    import torch
+
+    from . import octree as OT
+    from . import sdf as SD
+    f = np.float32
+    level = int(math.ceil(math.log2(float(f(f(inner_map_size) + f(2 * f(leaf_size))) * f(f(1.0) / f(leaf_size))))))
+    map_size = float(f(f(2 ** level) * f(leaf_size)))
+    pos = np.asarray(pos_W_M, np.float32)
+    wall = box_wall_points(leaf_size / 2, (-leaf_size, -leaf_size / 2, 0.0, leaf_size / 2, leaf_size))
+    xw = torch.from_numpy(wall).to(device)
+    pos_t = torch.from_numpy(pos).to(device)
+    m1p1 = ((xw - pos_t) * 2) * f(f(1.0) / f(map_size))  # SubMap::xyz_to_m1p1_pts
+    q = torch.unique(OT.quantize_points(m1p1, level), dim=0)
+    d = torch.tensor([[i, j, k] for i in (-1, 0, 1) for j in (-1, 0, 1) for k in (-1, 0, 1)], dtype=torch.int32, device=device)
+    q = (q.to(torch.int32)[:, None, :] + d[None]).view(-1, 3).clamp(0, 2 ** level - 1).to(torch.int16)  # points_to_neighbors + clamp
+    tree = OT.OctreeAS.from_quantized_points(q, level, device, origin=tuple(float(v) for v in pos), map_size=map_size)
+    net = SD.SdfNet(device, origin=tuple(float(v) for v in pos), map_size=map_size, seed=1337 + seed, mlp_mode=mlp_mode)
+    g = torch.Generator(device=device).manual_seed(seed)
+    opt = torch.optim.Adam([{"params": [net.params_], "lr": 1e-2}, {"params": [net.decoder_], "lr": 2e-3}], eps=1e-15)
+    b = torch.as_tensor(BOX, dtype=torch.float32, device=device)
+    for _ in range(steps):
+        # half the batch on the walls +- a 0.3 m band, half uniform in the room and around it
+        idx = torch.randint(0, xw.shape[0], (batch // 2,), device=device, generator=g)
+        near = xw[idx] + torch.randn(batch // 2, 3, device=device, generator=g) * 0.1
+        far = (torch.rand(batch // 2, 3, device=device, generator=g) * 2 - 1) * (b + 0.5)
+        x = torch.cat([near, far]).contiguous()
+        target = box_signed_distance(x)
+        sdf, _ = net.get_sdf(x)
+        loss = (sdf[:, 0] - target).abs().mean()
+        opt.zero_grad(set_to_none=False)
+        loss.backward()
+        opt.step()
+    lo = tuple(float(f(f(-0.5 * inner_map_size) + f(0.5 * leaf_size))) for _ in range(3))  # xyz_min_M_ + 0.5 * k_leaf_size (sub_map.cpp:17-18)
+    hi = tuple(float(f(f(0.5 * inner_map_size) - f(0.5 * leaf_size))) for _ in range(3))
+    return net, tree, (lo, hi)

@@ -1,0 +1,128 @@
+// gssdf::meshing_ (shim/include/gssdf_mesh.hpp) over the C ABI: the SubMap's members -> gssdf_sdf_mesh_args -> one gssdf_sdf_mesh call;
+// the counts are read back once and the call is repeated once with the exact counts if the first capacities were too small (as
+// gssdf_b200.mesh.meshing does).
+#include "gssdf_mesh.hpp"
+
+#include <ATen/cuda/CUDAContext.h>
+#include <c10/cuda/CUDAGuard.h>
+
+#include <cmath>
+#include <stdexcept>
+
+#include "../../include/gssdf_b200.h"
+
+namespace {
+void check(int rc) {
+    static const bool abi_ok = gssdf_abi_revision() == GSSDF_ABI_REVISION;
+    TORCH_CHECK(abi_ok, "gssdf_b200 meshing shim was compiled against ABI revision ", GSSDF_ABI_REVISION, " but libgssdf_b200.so is revision ",
+                gssdf_abi_revision(), ": rebuild the shim");
+    if (rc == GSSDF_EINVAL) throw std::invalid_argument(std::string("gssdf_b200: ") + gssdf_last_error());
+    if (rc != GSSDF_OK) throw std::runtime_error(std::string("gssdf_b200: ") + gssdf_last_error());
+}
+
+template <typename T>
+T cfg(const tcnn::cpp::json &j, const char *key, T dflt) {  // the defaults of the TCNNEncoding twin
+    return j.contains(key) ? j[key].get<T>() : dflt;
+}
+
+float at3(const torch::Tensor &t, int k) { return t.detach().to(torch::kCPU, torch::kFloat).contiguous().view({-1})[k].item<float>(); }
+}  // namespace
+
+std::vector<torch::Tensor> gssdf::meshing_(const torch::Tensor &octree_, const torch::Tensor &prefix_, const torch::Tensor &points_,
+                                           const torch::Tensor &pyramid_, int max_level_, const TCNNEncoding &encoder,
+                                           torch::nn::Sequential &decoder, const torch::Tensor &pos_W_M_,
+                                           const torch::Tensor &xyz_min_M_margin_, const torch::Tensor &xyz_max_M_margin_, float map_size,
+                                           float res, int vis_attribute, bool numerical_grad) {
+    torch::NoGradGuard no_grad;
+    TORCH_CHECK(octree_.is_cuda() && prefix_.is_cuda() && points_.is_cuda(), "octree_, prefix_ and points_ must be CUDA tensors");
+    TORCH_CHECK(octree_.scalar_type() == torch::kByte && prefix_.scalar_type() == torch::kInt && points_.scalar_type() == torch::kShort,
+                "octree_ uint8, prefix_ int32, points_ int16");
+    TORCH_CHECK(map_size > 0.f && res > 0.f, "map_size and res must be positive");
+    const c10::cuda::CUDAGuard guard(octree_.device());
+    const auto opt = torch::TensorOptions().device(octree_.device());
+    auto stream = reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream());
+
+    // the leaf-level rows of the point hierarchy: pyramid_[1][max_level_] onwards, pyramid_[0][max_level_] of them
+    auto pyr = pyramid_.detach().to(torch::kCPU, torch::kInt).contiguous().view({2, -1});
+    const int64_t n_leaves = pyr[0][max_level_].item<int>(), off = pyr[1][max_level_].item<int>();
+    torch::Tensor leaves = points_.slice(0, off, off + n_leaves).contiguous();
+
+    gssdf_sdf_mesh_args a{};
+    a.tree.level = max_level_;
+    a.tree.n_nodes = (int32_t)octree_.numel();
+    a.tree.octree = octree_.data_ptr<uint8_t>();
+    a.tree.exsum = prefix_.data_ptr<int32_t>();
+    a.tree.inv_size = (float)(1.0 / (double)map_size);  // k_map_size_inv as gssdf_b200.octree.OctreeAS computes it
+    a.tree.size = map_size;
+    a.leaves = leaves.data_ptr<int16_t>();
+    a.n_leaves = (int32_t)n_leaves;
+
+    // the net: encoder table -> fp16 shadow, decoder parameters flattened in torch::nn::Linear order (W[out,in] then bias, layer after layer)
+    const auto &c = encoder.encoding_config_;
+    gssdf_sdf_net &net = a.net;
+    net.n_levels = cfg<int>(c, "n_levels", 16);
+    net.n_features_per_level = cfg<int>(c, "n_features_per_level", 2);
+    net.log2_hashmap_size = cfg<int>(c, "log2_hashmap_size", 19);
+    net.base_resolution = cfg<int>(c, "base_resolution", 16);
+    net.per_level_scale = cfg<float>(c, "per_level_scale", 2.0f);
+    std::vector<torch::Tensor> ps;
+    for (auto &p : decoder->parameters()) ps.push_back(p.detach().to(opt.dtype(torch::kFloat)).flatten());
+    TORCH_CHECK(ps.size() >= 4 && ps.size() % 2 == 0, "decoder must be Linear / ReLU layers");
+    torch::Tensor mlp = torch::cat(ps).contiguous();
+    net.hidden_dim = (int32_t)ps[0].numel() / (int32_t)(net.n_levels * net.n_features_per_level);
+    net.n_hidden = (int32_t)ps.size() / 2 - 2;
+    net.mlp = mlp.data_ptr<float>();
+    torch::Tensor table = encoder.params_.detach().to(opt.dtype(torch::kFloat)).contiguous();
+    torch::Tensor half = torch::empty({table.numel()}, opt.dtype(torch::kHalf));
+    check(gssdf_sdf_table_to_half(table.data_ptr<float>(), half.data_ptr(), table.numel(), stream));
+    net.table_half = half.data_ptr();
+    TORCH_CHECK(gssdf_sdf_mlp_params(&net) == mlp.numel(), "decoder size does not match the encoder's output width");
+    for (int k = 0; k < 3; ++k) net.origin[k] = at3(pos_W_M_, k);
+    net.inv_size = (float)(1.0 / (double)map_size);
+    // decoder arithmetic as gssdf_b200.sdf.SdfNet chooses it: wgmma tensor cores where supported, else fp32 CUDA cores
+    torch::Tensor packed;
+    net.mlp_mode = (net.hidden_dim == 64 && net.n_hidden <= 3) ? 1 : 0;
+    if (net.mlp_mode == 1) {
+        packed = torch::empty({gssdf_sdf_mlp_packed_bytes(&net)}, opt.dtype(torch::kByte));
+        check(gssdf_sdf_mlp_pack(&net, packed.data_ptr(), stream));
+        net.mlp_packed = packed.data_ptr();
+    }
+
+    // the lattice of LocalMap::meshing_ for a box in one slab (local_map.cpp:248-253): fp32 bounds, ATen's arange length in double
+    for (int k = 0; k < 3; ++k) {
+        const float center = at3(pos_W_M_, k);
+        a.tree.origin[k] = center;
+        const float lo = at3(xyz_min_M_margin_, k) + center;
+        const float end = (at3(xyz_max_M_margin_, k) + center) + res;
+        a.lower[k] = lo;
+        a.n[k] = (int32_t)std::max(std::ceil(((double)end - (double)lo) / (double)res), 0.0);
+    }
+    a.res = res;
+    a.color_mode = vis_attribute == 0 ? 0 : (numerical_grad ? 2 : 1);
+
+    const int r = (int)std::ceil((double)map_size / (double)(1 << max_level_) / (double)res);
+    int64_t vcap = std::max<int64_t>(1024, 4 * n_leaves * (int64_t)(r + 1) * (r + 1)), fcap = 2 * vcap;
+    torch::Tensor counts = torch::zeros({4}, opt.dtype(torch::kInt));
+    a.counts = counts.data_ptr<int32_t>();
+    torch::Tensor ws;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        torch::Tensor vertices = torch::empty({std::max<int64_t>(vcap, 1), 3}, opt.dtype(torch::kFloat));
+        torch::Tensor faces = torch::empty({std::max<int64_t>(fcap, 1), 3}, opt.dtype(torch::kInt));
+        torch::Tensor colors = torch::empty({std::max<int64_t>(vcap, 1), 3}, opt.dtype(torch::kByte));
+        a.vertex_cap = vcap, a.face_cap = fcap;
+        a.vertices = vertices.data_ptr<float>();
+        a.faces = faces.data_ptr<int32_t>();
+        a.colors = colors.data_ptr<uint8_t>();
+        const size_t need = gssdf_sdf_mesh_workspace_bytes(&a);
+        if (!ws.defined() || (size_t)ws.numel() < need) ws = torch::empty({(int64_t)std::max<size_t>(need, 1)}, opt.dtype(torch::kByte));
+        a.workspace = ws.data_ptr();
+        a.workspace_bytes = (size_t)ws.numel();
+        check(gssdf_sdf_mesh(&a, stream));
+        auto h = counts.cpu();
+        const int32_t *cn = h.data_ptr<int32_t>();
+        TORCH_CHECK(!(cn[2] & 4), "gssdf_b200: meshing exceeded a per-leaf workspace bound");
+        if (!cn[2]) return {vertices.slice(0, 0, cn[0]), faces.slice(0, 0, cn[1]), colors.slice(0, 0, cn[0])};
+        vcap = cn[0], fcap = cn[1];
+    }
+    throw std::runtime_error("gssdf_b200: meshing overflowed its exact capacities");
+}

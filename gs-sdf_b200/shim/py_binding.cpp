@@ -6,6 +6,7 @@
 #include "gsplat_cpp/rasterize_to_pixels.h"
 #include "gsplat_cpp/rendering.h"
 #include "cumcubes.hpp"
+#include "gssdf_mesh.hpp"
 
 void bind_tcnn(pybind11::module &m);
 
@@ -13,6 +14,31 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     bind_tcnn(m);
     m.def("mc_marching_cubes", &mc::marching_cubes);
     m.def("mc_save_mesh_as_ply", &mc::save_mesh_as_ply);
+    // gssdf::meshing_ with LocalMap's decoder rebuilt from a flat parameter vector (torch::nn::Linear order), as local_map.cpp:29-42 builds it
+    m.def("gssdf_meshing_", [](const torch::Tensor &octree, const torch::Tensor &prefix, const torch::Tensor &points, const torch::Tensor &pyramid,
+                               int max_level, const std::shared_ptr<TCNNEncoding> &encoder, const torch::Tensor &decoder_flat, int hidden_dim,
+                               int geo_num_layer, const torch::Tensor &pos_W_M, const torch::Tensor &xyz_min_M_margin,
+                               const torch::Tensor &xyz_max_M_margin, float map_size, float res, int vis_attribute, bool numerical_grad) {
+        torch::nn::Sequential decoder;
+        decoder->push_back(torch::nn::Linear((int64_t)encoder->get_out_dim(), hidden_dim));
+        decoder->push_back(torch::nn::ReLU(true));
+        for (int i = 0; i < geo_num_layer; i++) {
+            decoder->push_back(torch::nn::Linear(hidden_dim, hidden_dim));
+            decoder->push_back(torch::nn::ReLU(true));
+        }
+        decoder->push_back(torch::nn::Linear(hidden_dim, 2));
+        decoder->to(decoder_flat.device());
+        {
+            torch::NoGradGuard ng;
+            int64_t o = 0;
+            for (auto &p : decoder->parameters()) {
+                p.copy_(decoder_flat.slice(0, o, o + p.numel()).view_as(p));
+                o += p.numel();
+            }
+        }
+        return gssdf::meshing_(octree, prefix, points, pyramid, max_level, *encoder, decoder, pos_W_M, xyz_min_M_margin, xyz_max_M_margin,
+                               map_size, res, vis_attribute, numerical_grad);
+    });
     m.def("fully_fused_projection_2dgs", &fully_fused_projection_2dgs);
     m.def("get_view_colors", [](const torch::Tensor &viewmats, const torch::Tensor &means, const torch::Tensor &radii,
                                 const torch::Tensor &colors, const torch::Tensor &camera_ids, const torch::Tensor &gaussian_ids,

@@ -49,7 +49,7 @@ const char *gssdf_last_error(void);
 /* "gssdf_b200 <ver> sm_90a" */
 const char *gssdf_version(void);
 /* Argument structs grow between revisions: a binding compiled against this header must see the same number from the library. */
-#define GSSDF_ABI_REVISION 15
+#define GSSDF_ABI_REVISION 16
 int32_t gssdf_abi_revision(void);
 
 /* L2 residency hint (SURVEY 7.6): marks [ptr, ptr+bytes) as a persisting access-policy window for kernels launched on `stream` from now on
@@ -889,6 +889,49 @@ typedef struct gssdf_marching_cubes_args {
 } gssdf_marching_cubes_args;
 size_t gssdf_marching_cubes_workspace_bytes(int32_t nx, int32_t ny, int32_t nz);
 int gssdf_marching_cubes(const gssdf_marching_cubes_args *a, gssdf_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * f-5  Meshing of a trained SDF in one call.  Replaces LocalMap::meshing_(float, bool) (include/neural_net/local_map.cpp:329-447)
+ *     on ONE global lattice: point i along axis k is lower[k] + i * res as torch.arange computes it on a CUDA tensor (one fp32 FMA),
+ *     i < n[k]. The field is the SDF (decoder output 0, the arithmetic of gssdf_sdf_fwd) at the lattice points the octree marks as
+ *     occupied (gssdf_octree_query) and 1e-6 elsewhere; marching cubes with thresh 0 on it (upper = lower + n * res, the vertex
+ *     arithmetic of gssdf_marching_cubes) visits only cells with an occupied corner, which is exact: before filtering the mesh equals
+ *     gssdf_marching_cubes on the dense field, vertex for vertex and face for face. Then the reference's boundary filter (a vertex
+ *     passes iff the 27 points (floor(v / res) + d) * res, d in {-1,0,1}^3, are all occupied; a face is kept iff its three vertices
+ *     pass), and compaction: faces keep their order, vertices no kept face references are dropped and the rest renumbered in order.
+ *     Work follows the occupied leaves: one CTA per leaf queries a brick of lattice points around it, so the SDF is evaluated at the
+ *     occupied lattice points only, each once. No host sync, no allocation; writes stop at the capacities and the true counts are
+ *     reported (as in gssdf_marching_cubes).
+ *     Workspace per leaf: 70-94 bytes per work-point slot ((ceil(leaf / res) + 2)^3 slots) plus 16 bytes per occupied-point slot
+ *     ((ceil(leaf / res) + 1)^3), plus CUB's temporary storage for the key sort and the scans, plus the colour buffers (16 or 28 bytes
+ *     per vertex of vertex_cap for colour modes 1 / 2); DESIGN 7f itemises it. gssdf_sdf_mesh_workspace_bytes gives the exact size.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct gssdf_sdf_mesh_args {
+    gssdf_octree tree;            /* occupancy: tree.origin = pos_W_M, tree.inv_size = 1 / k_map_size (world coordinates) */
+    const int16_t *leaves;        /* device [n_leaves,3]: every leaf-level row of the point hierarchy (OctreeAS::points_ from pyramid_
+                                     offset max_level_), each once */
+    int32_t n_leaves;
+    gssdf_sdf_net net;            /* either mlp_mode */
+    float lower[3];               /* xyz_min_M_margin + pos_W_M in fp32 */
+    int32_t n[3];                 /* lattice points per axis: the length of torch::arange(lower, max_margin + center + res, res) */
+    float res;                    /* > 0; |coordinate / res| + 1 must fit int16 (the filter's cast), GSSDF_EINVAL otherwise */
+    int32_t color_mode;           /* 0: 127 grey (c = 0.5); 1: analytic normal (gssdf_sdf_bwd, v_sdf = 1); 2: numerical normal
+                                     (gssdf_sdf_fwd, 7 variants, delta = res). colors = (c * 255).to(uint8), c = normalize(grad) / 2 + 0.5.
+                                     Mode 1 inherits gssdf_sdf_bwd's order-dependent sum of the per-level input gradients (shared-memory
+                                     atomics): repeated calls agree to within 1 per channel; everything else is identical call to call */
+    int64_t vertex_cap, face_cap; /* rows allocated in vertices (and colors) / faces */
+    float *vertices;              /* [vertex_cap,3] */
+    int32_t *faces;               /* [face_cap,3] */
+    uint8_t *colors;              /* [vertex_cap,3] or NULL */
+    int32_t *counts;              /* device int32[4], overwritten: V, F, overflow bits (1 vertices, 2 faces, 4 a per-leaf workspace bound,
+                                     which the lattice geometry should never exceed), number of lattice points whose SDF was evaluated */
+    void *workspace;              /* >= gssdf_sdf_mesh_workspace_bytes(a) */
+    size_t workspace_bytes;
+} gssdf_sdf_mesh_args;
+/* reads tree.level, tree.inv_size, n_leaves, n[3], res, color_mode and vertex_cap of *a; 0 when any of them is invalid (res <= 0,
+   any n <= 0, a level outside [1, 15], or a lattice that could give more than 2^31 - 1 faces) */
+size_t gssdf_sdf_mesh_workspace_bytes(const gssdf_sdf_mesh_args *a);
+int gssdf_sdf_mesh(const gssdf_sdf_mesh_args *a, gssdf_stream_t stream);
 
 #ifdef __cplusplus
 }
