@@ -2,6 +2,7 @@
 // the counts are read back once and the call is repeated once with the exact counts if the first capacities were too small (as
 // gssdf_b200.mesh.meshing does).
 #include "gssdf_mesh.hpp"
+#include "gssdf_sdf_net.hpp"
 
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -27,6 +28,42 @@ T cfg(const tcnn::cpp::json &j, const char *key, T dflt) {  // the defaults of t
 
 float at3(const torch::Tensor &t, int k) { return t.detach().to(torch::kCPU, torch::kFloat).contiguous().view({-1})[k].item<float>(); }
 }  // namespace
+
+gssdf::SdfNetHolder gssdf::make_sdf_net(const TCNNEncoding &encoder, torch::nn::Sequential &decoder, const torch::Tensor &pos_W_M_,
+                                        float map_size, gssdf_stream_t stream) {
+    const auto opt = torch::TensorOptions().device(encoder.params_.device());
+    SdfNetHolder h;
+    // the net: encoder table -> fp16 shadow, decoder parameters flattened in torch::nn::Linear order (W[out,in] then bias, layer after layer)
+    const auto &c = encoder.encoding_config_;
+    gssdf_sdf_net &net = h.net;
+    net.n_levels = cfg<int>(c, "n_levels", 16);
+    net.n_features_per_level = cfg<int>(c, "n_features_per_level", 2);
+    net.log2_hashmap_size = cfg<int>(c, "log2_hashmap_size", 19);
+    net.base_resolution = cfg<int>(c, "base_resolution", 16);
+    net.per_level_scale = cfg<float>(c, "per_level_scale", 2.0f);
+    std::vector<torch::Tensor> ps;
+    for (auto &p : decoder->parameters()) ps.push_back(p.detach().to(opt.dtype(torch::kFloat)).flatten());
+    TORCH_CHECK(ps.size() >= 4 && ps.size() % 2 == 0, "decoder must be Linear / ReLU layers");
+    h.mlp = torch::cat(ps).contiguous();
+    net.hidden_dim = (int32_t)ps[0].numel() / (int32_t)(net.n_levels * net.n_features_per_level);
+    net.n_hidden = (int32_t)ps.size() / 2 - 2;
+    net.mlp = h.mlp.data_ptr<float>();
+    torch::Tensor table = encoder.params_.detach().to(opt.dtype(torch::kFloat)).contiguous();
+    h.half = torch::empty({table.numel()}, opt.dtype(torch::kHalf));
+    check(gssdf_sdf_table_to_half(table.data_ptr<float>(), h.half.data_ptr(), table.numel(), stream));
+    net.table_half = h.half.data_ptr();
+    TORCH_CHECK(gssdf_sdf_mlp_params(&net) == h.mlp.numel(), "decoder size does not match the encoder's output width");
+    for (int k = 0; k < 3; ++k) net.origin[k] = at3(pos_W_M_, k);
+    net.inv_size = (float)(1.0 / (double)map_size);
+    // decoder arithmetic as gssdf_b200.sdf.SdfNet chooses it: wgmma tensor cores where supported, else fp32 CUDA cores
+    net.mlp_mode = (net.hidden_dim == 64 && net.n_hidden <= 3) ? 1 : 0;
+    if (net.mlp_mode == 1) {
+        h.packed = torch::empty({gssdf_sdf_mlp_packed_bytes(&net)}, opt.dtype(torch::kByte));
+        check(gssdf_sdf_mlp_pack(&net, h.packed.data_ptr(), stream));
+        net.mlp_packed = h.packed.data_ptr();
+    }
+    return h;
+}
 
 std::vector<torch::Tensor> gssdf::meshing_(const torch::Tensor &octree_, const torch::Tensor &prefix_, const torch::Tensor &points_,
                                            const torch::Tensor &pyramid_, int max_level_, const TCNNEncoding &encoder,
@@ -57,36 +94,8 @@ std::vector<torch::Tensor> gssdf::meshing_(const torch::Tensor &octree_, const t
     a.leaves = leaves.data_ptr<int16_t>();
     a.n_leaves = (int32_t)n_leaves;
 
-    // the net: encoder table -> fp16 shadow, decoder parameters flattened in torch::nn::Linear order (W[out,in] then bias, layer after layer)
-    const auto &c = encoder.encoding_config_;
-    gssdf_sdf_net &net = a.net;
-    net.n_levels = cfg<int>(c, "n_levels", 16);
-    net.n_features_per_level = cfg<int>(c, "n_features_per_level", 2);
-    net.log2_hashmap_size = cfg<int>(c, "log2_hashmap_size", 19);
-    net.base_resolution = cfg<int>(c, "base_resolution", 16);
-    net.per_level_scale = cfg<float>(c, "per_level_scale", 2.0f);
-    std::vector<torch::Tensor> ps;
-    for (auto &p : decoder->parameters()) ps.push_back(p.detach().to(opt.dtype(torch::kFloat)).flatten());
-    TORCH_CHECK(ps.size() >= 4 && ps.size() % 2 == 0, "decoder must be Linear / ReLU layers");
-    torch::Tensor mlp = torch::cat(ps).contiguous();
-    net.hidden_dim = (int32_t)ps[0].numel() / (int32_t)(net.n_levels * net.n_features_per_level);
-    net.n_hidden = (int32_t)ps.size() / 2 - 2;
-    net.mlp = mlp.data_ptr<float>();
-    torch::Tensor table = encoder.params_.detach().to(opt.dtype(torch::kFloat)).contiguous();
-    torch::Tensor half = torch::empty({table.numel()}, opt.dtype(torch::kHalf));
-    check(gssdf_sdf_table_to_half(table.data_ptr<float>(), half.data_ptr(), table.numel(), stream));
-    net.table_half = half.data_ptr();
-    TORCH_CHECK(gssdf_sdf_mlp_params(&net) == mlp.numel(), "decoder size does not match the encoder's output width");
-    for (int k = 0; k < 3; ++k) net.origin[k] = at3(pos_W_M_, k);
-    net.inv_size = (float)(1.0 / (double)map_size);
-    // decoder arithmetic as gssdf_b200.sdf.SdfNet chooses it: wgmma tensor cores where supported, else fp32 CUDA cores
-    torch::Tensor packed;
-    net.mlp_mode = (net.hidden_dim == 64 && net.n_hidden <= 3) ? 1 : 0;
-    if (net.mlp_mode == 1) {
-        packed = torch::empty({gssdf_sdf_mlp_packed_bytes(&net)}, opt.dtype(torch::kByte));
-        check(gssdf_sdf_mlp_pack(&net, packed.data_ptr(), stream));
-        net.mlp_packed = packed.data_ptr();
-    }
+    const SdfNetHolder holder = make_sdf_net(encoder, decoder, pos_W_M_, map_size, stream);
+    a.net = holder.net;
 
     // the lattice of LocalMap::meshing_ for a box in one slab (local_map.cpp:248-253): fp32 bounds, ATen's arange length in double
     for (int k = 0; k < 3; ++k) {

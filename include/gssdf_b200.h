@@ -49,7 +49,7 @@ const char *gssdf_last_error(void);
 /* "gssdf_b200 <ver> sm_90a" */
 const char *gssdf_version(void);
 /* Argument structs grow between revisions: a binding compiled against this header must see the same number from the library. */
-#define GSSDF_ABI_REVISION 16
+#define GSSDF_ABI_REVISION 17
 int32_t gssdf_abi_revision(void);
 
 /* L2 residency hint (SURVEY 7.6): marks [ptr, ptr+bytes) as a persisting access-policy window for kernels launched on `stream` from now on
@@ -932,6 +932,54 @@ typedef struct gssdf_sdf_mesh_args {
    any n <= 0, a level outside [1, 15], or a lattice that could give more than 2^31 - 1 faces) */
 size_t gssdf_sdf_mesh_workspace_bytes(const gssdf_sdf_mesh_args *a);
 int gssdf_sdf_mesh(const gssdf_sdf_mesh_args *a, gssdf_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * f-6  Splat initialisation from the trained SDF.  Replaces init_gs_with_sdf(local_map, xyzs, mesh_res, init_opa)
+ *     (include/neural_gaussian/neural_gaussian.cpp:19-127), which NeuralGS::NeuralGS calls on the mesh vertices (:322-326).
+ *     The reference's get_gradient(xyzs, mesh_res, {}, true) takes its numerical branch (_numerical_grad defaults to true,
+ *     include/neural_net/local_map.h:41-45): grad is the 6-offset central difference and curv_dom the numerical Hessian diagonal
+ *     (local_map.cpp:110-146). All SDF values come from ONE gssdf_sdf_fwd(n_variants = 7, delta) on the points (bit-identical to that
+ *     operator; variant 0 equals an n_variants = 1 launch), then ONE epilogue kernel, one thread per point, restates the ATen sequence
+ *     operation by operation, each rounded once as ATen's separate kernels round it:
+ *       grad     = fl32(0.5 * inv_delta) * (s[+k] - s[-k]),   inv_delta = 1.0 / delta in double
+ *       curv_dom = fl32(inv_delta * inv_delta) * ((s[+k] + s[-k]) - 2 s)
+ *       quaternion = rot6d_to_quat(normalize(grad), normalize(curv_dom))            (normalize: eps 1e-12, NaN propagates)
+ *       opacity  = exp(-s^2 * isigma),  isigma = 1 + softplus_100(y1) * bce_isigma   (ATen softplus: x*100 > 20 ? x : log1p(exp(100 x)) / 100)
+ *     rot6d_to_quat (utils::rotation_6d_to_matrix, include/utils/utils.cpp:693-719, then neural_gaussian.cpp:68-100): b1 = normalize(a1),
+ *     b2 = normalize(a2 - (b1.a2) b1), b3 = b1 x b2; columns permuted to [b2, b3, b1] (the splat's z axis is b1); angle =
+ *     acos((trace - 1) * 0.5); axis = normalize((R21 - R12, R02 - R20, R10 - R01) / (2 sin angle)); q = (cos(angle/2), sin(angle/2) axis);
+ *     nan_to_num (NaN -> 0, +-inf -> +-FLT_MAX). Quirks kept: an acos argument past +-1 by rounding gives q = 0; angle 0 gives (1,0,0,0);
+ *     near angle pi the axis is rounding noise / sin(angle) and as arbitrary as the reference's. Precise acosf / sinf / cosf / expf /
+ *     log1pf, as ATen's kernels call them. No host sync, no allocation; rows >= *n_live are untouched; n == 0 is a no-op.
+ *     GSSDF_EINVAL before any launch for n < 0, delta <= 0 or non-finite, a NULL quaternion or a workspace that is too small.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct gssdf_sdf_init_gs_args {
+    gssdf_sdf_net net;            /* either mlp_mode */
+    int64_t n;                    /* points */
+    const float *x;               /* [n,3] world frame, as in gssdf_sdf_fwd */
+    const int32_t *n_live;        /* device int32 or NULL: rows >= min(n, *n_live) stay untouched */
+    float delta;                  /* mesh_res: the offset of the central differences, > 0 */
+    float bce_isigma;             /* k_bce_isigma = 1 / bce_sigma (params.cpp:197) */
+    float *grad;                  /* [n,3] or NULL */
+    float *curv_dom;              /* [n,3] or NULL */
+    float *quaternion;            /* [n,4] (w, x, y, z) */
+    float *opacity;               /* [n] or NULL (init_opa == false) */
+    void *workspace;              /* >= gssdf_sdf_init_gs_workspace_bytes(n): the 7n SDF values and decoder outputs 1 */
+    size_t workspace_bytes;
+} gssdf_sdf_init_gs_args;
+/* 0 for n < 0 */
+size_t gssdf_sdf_init_gs_workspace_bytes(int64_t n);
+int gssdf_sdf_init_gs(const gssdf_sdf_init_gs_args *a, gssdf_stream_t stream);
+
+/* The rot6d_to_quat step above on its own (the same device function), from b1 = normalize(a1) onward: the sky splats' quaternions
+   (neural_gaussian.cpp:363-392, a1 = sphere samples, a2 = their (y, z, x)). GSSDF_EINVAL for n < 0 or a NULL quaternion. */
+typedef struct gssdf_rot6d_to_quat_args {
+    int64_t n;
+    const float *a1, *a2;         /* [n,3] each */
+    const int32_t *n_live;        /* device int32 or NULL */
+    float *quaternion;            /* [n,4] */
+} gssdf_rot6d_to_quat_args;
+int gssdf_rot6d_to_quat(const gssdf_rot6d_to_quat_args *a, gssdf_stream_t stream);
 
 #ifdef __cplusplus
 }
