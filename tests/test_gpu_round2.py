@@ -327,9 +327,10 @@ def test_adam_step_matches_torch_adam():
 
 # ------------------------------------------------------------------------------------------------------------------------------
 def _depth_to_normal_ref(depth, V, K):
-    """sensor::depth_to_normal (cameras.hpp:176-226) in torch fp64: depth [H,W,1], V world->camera [4,4], K [3,3]."""
+    """sensor::depth_to_normal (cameras.hpp:176-226) in torch, in depth's precision (fp64 as the reference arbiter): depth [H,W,1],
+    V world->camera [4,4], K [3,3] of the same dtype."""
     H, W = depth.shape[:2]
-    ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
+    ys, xs = torch.meshgrid(torch.arange(H, dtype=depth.dtype), torch.arange(W, dtype=depth.dtype), indexing="ij")
     zdir = torch.stack([(xs + 0.5 - K[0, 2]) / K[0, 0], (ys + 0.5 - K[1, 2]) / K[1, 1], torch.ones_like(xs)], -1)
     rot = V[:3, :3].T  # camera -> world
     pos = -rot @ V[:3, 3]
