@@ -111,3 +111,86 @@ def meshing(tree, net, xyz_min_margin, xyz_max_margin, res, color_mode=0, vertex
                 return vertices[:nv], faces[:nf], colors[:nv]
             vcap, fcap = nv, nf
     raise RuntimeError("gssdf_b200: meshing overflowed its exact capacities")
+
+
+def cull_vertices(vertices, w2c, depths, fx, fy, cx, cy, W, H, seen):
+    """Raw gssdf_mesh_cull_vertices: ORs the visibility of the frames w2c [B,4,4] / depths [B,Hd,Wd] (CUDA float32; rows may be
+    padded, frames Hd rows apart) into seen (CUDA uint8 [N], in place). vertices: CUDA float32 [N,3]."""
+    B, Hd, Wd = depths.shape
+    if depths.dtype != torch.float32 or not depths.is_cuda or depths.stride(2) != 1 or depths.stride(0) != Hd * depths.stride(1):
+        raise ValueError("gssdf_b200: depths must be a CUDA float32 [B,Hd,Wd] with unit column stride and frames Hd rows apart")
+    a = make_args("gssdf_mesh_cull_vertices_args", n=vertices.shape[0], vertices=vertices, n_frames=B, w2c=w2c, depth=depths,
+                  depth_h=Hd, depth_w=Wd, depth_row_stride=depths.stride(1), fx=float(fx), fy=float(fy), cx=float(cx), cy=float(cy),
+                  width=int(W), height=int(H), seen=seen)
+    check(lib().gssdf_mesh_cull_vertices(C.byref(a), cabi._stream()))
+
+
+def cull_faces(faces, n_vertices, seen, out, counts, ws):
+    """Raw gssdf_mesh_cull_faces: the faces (CUDA int32 [M,3]) with a seen vertex into out [M,3], stable; counts (CUDA int32 [2]) gets
+    [kept, error bits]."""
+    m = faces.shape[0]
+    w = ws.get(lib().gssdf_mesh_cull_workspace_bytes(m))
+    a = make_args("gssdf_mesh_cull_faces_args", m=m, faces=faces, n_vertices=n_vertices, seen=seen, out=out, counts=counts, workspace=w,
+                  workspace_bytes=w.numel())
+    check(lib().gssdf_mesh_cull_faces(C.byref(a), cabi._stream()))
+
+
+def depth_frames(depths):
+    """[B,Hd,Wd] or [B,Hd,Wd,1] (the reference's get_depth_image layout, stacked) float32 -> [B,Hd,Wd] view."""
+    if depths.dim() == 4 and depths.shape[-1] == 1:
+        depths = depths[..., 0]
+    if depths.dim() != 3 or depths.dtype != torch.float32:
+        raise ValueError(f"gssdf_b200: depths must be float32 [B,Hd,Wd] or [B,Hd,Wd,1], got {depths.dtype} {tuple(depths.shape)}")
+    return depths
+
+
+def camera_from_K(K):
+    """(fx, fy, cx, cy) as fp32 values from the reference's K = [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] (mesher.cpp:83-89)."""
+    k = np.asarray(K.detach().cpu() if hasattr(K, "detach") else K, np.float32).reshape(3, 3)
+    if k[0, 1] != 0 or k[1, 0] != 0 or k[2].tolist() != [0.0, 0.0, 1.0]:
+        raise ValueError(f"gssdf_b200: K must be [[fx, 0, cx], [0, fy, cy], [0, 0, 1]], got {k.tolist()}")
+    return float(k[0, 0]), float(k[1, 1]), float(k[0, 2]), float(k[1, 2])
+
+
+def cull_mesh(vertices, faces, depths, c2w, K, W, H, chunk=None, seen=None):
+    """Mesher::cull_mesh (include/mesher/mesher.cpp:76-160) on the GPU (DESIGN 7h). vertices: CUDA float32 [N,3]; faces: CUDA int32 [M,3];
+    depths: float32 [B,Hd,Wd] or [B,Hd,Wd,1] on the CPU or the GPU (the image need not be H x W); c2w: [B,4,4] camera->world poses,
+    inverted on the host with torch.inverse as in the reference; K: the 3x3 pinhole matrix; W, H: the camera's image size.
+    A vertex is seen if some frame has it at z >= 0, inside (0, W) x (0, H), and not more than 0.02 behind the bilinearly sampled depth;
+    a face is kept if one of its vertices is seen, in order. Frames go to the kernel `chunk` at a time (default: as many as fill half of
+    the L2 cache, so a chunk of images stays resident while every vertex walks it). seen: CUDA uint8 [N] to continue from (updated in
+    place) for callers that stream frames over several calls; None starts from nothing seen. The kept count is read back once.
+    Returns (vertices, kept faces [K,3] int32 -- [1,3] when one face is kept, where the reference's squeeze gives [3] --, seen)."""
+    v = cabi._req(vertices, torch.float32, "vertices")
+    f = cabi._req(faces, torch.int32, "faces")
+    if v.dim() != 2 or v.shape[1] != 3 or f.dim() != 2 or f.shape[1] != 3:
+        raise ValueError(f"gssdf_b200: vertices and faces must be [N,3] and [M,3], got {tuple(v.shape)} and {tuple(f.shape)}")
+    d = depth_frames(depths)
+    pose = c2w.detach().to("cpu", torch.float32)
+    if pose.dim() != 3 or pose.shape[1:] != (4, 4) or pose.shape[0] != d.shape[0]:
+        raise ValueError(f"gssdf_b200: c2w must be [B,4,4] with B = {d.shape[0]} depth frames, got {tuple(pose.shape)}")
+    if int(W) <= 0 or int(H) <= 0:
+        raise ValueError(f"gssdf_b200: W and H must be positive, got {W} x {H}")
+    fx, fy, cx, cy = camera_from_K(K)
+    dev, n, B = v.device, v.shape[0], d.shape[0]
+    if seen is None:
+        seen = torch.zeros(n, dtype=torch.uint8, device=dev)
+    elif not (seen.is_cuda and seen.dtype == torch.uint8 and seen.shape == (n,) and seen.is_contiguous()):
+        raise ValueError("gssdf_b200: seen must be a contiguous CUDA uint8 [N]")
+    if chunk is None:
+        frame_bytes = max(d.shape[1] * d.shape[2] * 4, 1)
+        chunk = max(1, torch.cuda.get_device_properties(dev).L2_cache_size // 2 // frame_bytes)
+    w2c = torch.inverse(pose).to(dev).contiguous()
+    for b0 in range(0, B, int(chunk)):
+        dc = d[b0:b0 + int(chunk)].to(dev)
+        if dc.stride(2) != 1 or dc.stride(0) != dc.shape[1] * dc.stride(1):
+            dc = dc.contiguous()
+        cull_vertices(v, w2c[b0:b0 + int(chunk)], dc, fx, fy, cx, cy, W, H, seen)
+    out = torch.empty(max(f.shape[0], 1), 3, dtype=torch.int32, device=dev)
+    counts = torch.empty(2, dtype=torch.int32, device=dev)
+    cull_faces(f, n, seen, out, counts, cabi.Workspace(dev))
+    kept, err = counts.tolist()
+    if err & 1:
+        bad = f[(f < 0) | (f >= n)][0]
+        raise IndexError(f"index {int(bad)} is out of bounds for dimension 0 with size {n}")
+    return v, out[:kept], seen

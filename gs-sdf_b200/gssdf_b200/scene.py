@@ -162,3 +162,60 @@ def box_room_sdf_net(device, inner_map_size=14.0, leaf_size=0.05, steps=1000, se
     lo = tuple(float(f(f(-0.5 * inner_map_size) + f(0.5 * leaf_size))) for _ in range(3))  # xyz_min_M_ + 0.5 * k_leaf_size (sub_map.cpp:17-18)
     hi = tuple(float(f(f(0.5 * inner_map_size) - f(0.5 * leaf_size))) for _ in range(3))
     return net, tree, (lo, hi)
+
+
+# an occluding pillar for the culling scenes: floor to ceiling, NOT part of box_room_sdf_net's SDF, in front of the cameras' cluster
+PILLAR_MIN = np.array([0.5, -0.3, -BOX[2]], np.float64)
+PILLAR_MAX = np.array([1.1, 0.3, BOX[2]], np.float64)
+CULL_CAM_CENTER = np.array([-1.5, 0.0, 0.0], np.float64)
+
+
+def box_room_cull_poses(n, seed=0, radius=0.1, max_yaw=math.radians(50.0), max_pitch=0.2):
+    """c2w [n,4,4] float32 (OpenCV axes: x right, y down, z forward) for the culling scenes: positions within `radius` of
+    CULL_CAM_CENTER, looking toward +x with |yaw| <= max_yaw, so the -x wall behind them is never in view, and the pillar hides the
+    same patch of the +x wall from all of them."""
+    rng = np.random.default_rng(seed)
+    out = np.zeros((n, 4, 4))
+    for i in range(n):
+        d = rng.normal(size=3)
+        pos = CULL_CAM_CENTER + radius * rng.uniform() ** (1 / 3) * d / np.linalg.norm(d)
+        yaw, pitch = rng.uniform(-max_yaw, max_yaw), rng.uniform(-max_pitch, max_pitch)
+        f = np.array([math.cos(pitch) * math.cos(yaw), math.cos(pitch) * math.sin(yaw), math.sin(pitch)])
+        right = np.cross(f, [0.0, 0.0, 1.0])
+        right /= np.linalg.norm(right)
+        down = np.cross(f, right)
+        out[i, :3, :3] = np.stack([right, down, f], 1)
+        out[i, :3, 3] = pos
+        out[i, 3, 3] = 1.0
+    return out.astype(np.float32)
+
+
+def box_room_depth(c2w, fx, fy, cx, cy, W, H, pillar=True, batch=16):
+    """Analytic z-depth images [B,H,W,1] float32 of the BOX room's inner walls (plus the occluding pillar) seen from the c2w poses
+    [B,4,4] (torch, any device; rendered there `batch` frames at a time), pixel (i, j) along K^-1 [j, i, 1], as the reference's
+    get_depth_image hands them to Mesher::cull_mesh. Test and benchmark infrastructure."""
+    import torch
+    dev = c2w.device
+    j = torch.arange(W, dtype=torch.float64, device=dev)
+    i = torch.arange(H, dtype=torch.float64, device=dev)
+    dc = torch.stack([((j[None, :] - cx) / fx).expand(H, W), ((i[:, None] - cy) / fy).expand(H, W), torch.ones(H, W, dtype=torch.float64,
+                                                                                                             device=dev)], -1)
+    box = torch.as_tensor(BOX, dtype=torch.float64, device=dev)
+    pmin = torch.as_tensor(PILLAR_MIN, dtype=torch.float64, device=dev)
+    pmax = torch.as_tensor(PILLAR_MAX, dtype=torch.float64, device=dev)
+    out = []
+    for b0 in range(0, c2w.shape[0], batch):
+        P = c2w[b0:b0 + batch].to(torch.float64)
+        o = P[:, None, None, :3, 3]
+        d = torch.einsum("brc,hwc->bhwr", P[:, :3, :3], dc)  # world direction with camera z = 1, so the ray parameter is the z-depth
+        with torch.no_grad():
+            t_wall = torch.where(d > 0, (box - o) / d, torch.where(d < 0, (-box - o) / d, torch.full_like(d, float("inf")))).amin(-1)
+            t = t_wall
+            if pillar:
+                t1, t2 = (pmin - o) / d, (pmax - o) / d
+                t_in = torch.minimum(t1, t2).amax(-1)
+                t_out = torch.maximum(t1, t2).amin(-1)
+                hit = (t_in <= t_out) & (t_in > 0)
+                t = torch.where(hit, torch.minimum(t_in, t_wall), t_wall)
+        out.append(t.to(torch.float32)[..., None])
+    return torch.cat(out, 0)

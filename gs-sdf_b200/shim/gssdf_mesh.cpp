@@ -135,3 +135,71 @@ std::vector<torch::Tensor> gssdf::meshing_(const torch::Tensor &octree_, const t
     }
     throw std::runtime_error("gssdf_b200: meshing overflowed its exact capacities");
 }
+
+void gssdf::cull_mesh_accumulate(torch::Tensor &seen, const torch::Tensor &vertices, const torch::Tensor &depths, const torch::Tensor &c2w,
+                                 float fx, float fy, float cx, float cy, int W, int H) {
+    torch::NoGradGuard no_grad;
+    TORCH_CHECK(seen.is_cuda() && seen.scalar_type() == torch::kByte && seen.dim() == 1 && seen.is_contiguous(),
+                "seen must be a contiguous CUDA uint8 [N]");
+    TORCH_CHECK(vertices.dim() == 2 && vertices.size(1) == 3 && vertices.size(0) == seen.size(0) && vertices.scalar_type() == torch::kFloat,
+                "vertices must be float32 [N,3] with N = seen.size(0)");
+    torch::Tensor d = (depths.dim() == 4 && depths.size(3) == 1) ? depths.select(3, 0) : depths;
+    TORCH_CHECK(d.dim() == 3 && d.scalar_type() == torch::kFloat, "depths must be float32 [B,Hd,Wd,1] or [B,Hd,Wd]");
+    TORCH_CHECK(c2w.dim() == 3 && c2w.size(0) == d.size(0) && c2w.size(1) == 4 && c2w.size(2) == 4, "c2w must be [B,4,4] with B = depths.size(0)");
+    const c10::cuda::CUDAGuard guard(seen.device());
+    auto stream = reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream());
+    const auto dev = seen.device();
+    torch::Tensor v = vertices.to(dev).contiguous();
+    torch::Tensor w2c = torch::inverse(c2w.to(torch::kCPU, torch::kFloat)).to(dev).contiguous();
+    d = d.to(dev);
+    if (d.stride(2) != 1 || d.stride(0) != d.size(1) * d.stride(1)) d = d.contiguous();
+    gssdf_mesh_cull_vertices_args a{};
+    a.n = v.size(0);
+    a.vertices = v.data_ptr<float>();
+    a.n_frames = (int32_t)d.size(0);
+    a.w2c = w2c.data_ptr<float>();
+    a.depth = d.data_ptr<float>();
+    a.depth_h = (int32_t)d.size(1), a.depth_w = (int32_t)d.size(2);
+    a.depth_row_stride = d.stride(1);
+    a.fx = fx, a.fy = fy, a.cx = cx, a.cy = cy;
+    a.width = W, a.height = H;
+    a.seen = seen.data_ptr<uint8_t>();
+    check(gssdf_mesh_cull_vertices(&a, stream));
+}
+
+torch::Tensor gssdf::cull_mesh_faces(const torch::Tensor &faces, const torch::Tensor &seen) {
+    torch::NoGradGuard no_grad;
+    TORCH_CHECK(seen.is_cuda() && seen.scalar_type() == torch::kByte && seen.dim() == 1 && seen.is_contiguous(),
+                "seen must be a contiguous CUDA uint8 [N]");
+    TORCH_CHECK(faces.dim() == 2 && faces.size(1) == 3 && (faces.scalar_type() == torch::kInt || faces.scalar_type() == torch::kLong),
+                "faces must be int32 or int64 [M,3]");
+    const int64_t n = seen.size(0);
+    auto bad_index = [&](const torch::Tensor &f) {
+        const int64_t bad = f.masked_select((f < 0) | (f >= n)).flatten()[0].item<int64_t>();
+        TORCH_CHECK_INDEX(false, "index ", bad, " is out of bounds for dimension 0 with size ", n);
+    };
+    // int64 ids that do not fit int32 cannot be narrowed for the kernel: they are out of range for any seen[] the library accepts
+    if (faces.scalar_type() == torch::kLong && ((faces < 0) | (faces >= n)).any().item<bool>()) bad_index(faces);
+    const c10::cuda::CUDAGuard guard(seen.device());
+    auto stream = reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream());
+    const auto opt = torch::TensorOptions().device(seen.device());
+    torch::Tensor f = faces.to(opt.dtype(torch::kInt)).contiguous();
+    const int64_t m = f.size(0);
+    torch::Tensor out = torch::empty({std::max<int64_t>(m, 1), 3}, opt.dtype(torch::kInt));
+    torch::Tensor counts = torch::empty({2}, opt.dtype(torch::kInt));
+    torch::Tensor ws = torch::empty({(int64_t)std::max<size_t>(gssdf_mesh_cull_workspace_bytes(m), 1)}, opt.dtype(torch::kByte));
+    gssdf_mesh_cull_faces_args a{};
+    a.m = m;
+    a.faces = f.data_ptr<int32_t>();
+    a.n_vertices = n;
+    a.seen = seen.data_ptr<uint8_t>();
+    a.out = out.data_ptr<int32_t>();
+    a.counts = counts.data_ptr<int32_t>();
+    a.workspace = ws.data_ptr();
+    a.workspace_bytes = (size_t)ws.numel();
+    check(gssdf_mesh_cull_faces(&a, stream));
+    auto h = counts.cpu();
+    const int32_t *cn = h.data_ptr<int32_t>();
+    if (cn[1] & 1) bad_index(f);
+    return out.slice(0, 0, cn[0]).to(faces.device(), faces.scalar_type());
+}

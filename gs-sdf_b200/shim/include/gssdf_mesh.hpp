@@ -20,4 +20,15 @@ std::vector<torch::Tensor> meshing_(const torch::Tensor &octree_, const torch::T
                                     torch::nn::Sequential &decoder, const torch::Tensor &pos_W_M_, const torch::Tensor &xyz_min_M_margin_,
                                     const torch::Tensor &xyz_max_M_margin_, float map_size, float res, int vis_attribute,
                                     bool numerical_grad);
+
+// Mesher::cull_mesh (include/mesher/mesher.cpp:76-160) in two calls (gssdf_mesh_cull_vertices / _faces; DESIGN 7h, INTEGRATION 3e).
+// cull_mesh_accumulate ORs the visibility of one batch of depth frames into seen (contiguous CUDA uint8 [N], zeros to start):
+// vertices [N,3] float32 on the CPU (as Mesher holds them) or on seen's device; depths [B,Hd,Wd,1] or [B,Hd,Wd] float32 and c2w [B,4,4]
+// (get_depth_image / get_pose(i, RawDepth) stacked, any device; the poses are inverted on the host with torch::inverse, as the reference
+// does); fx, fy, cx, cy, W, H: the sensor's camera. Batches may come in any size and order.
+void cull_mesh_accumulate(torch::Tensor &seen, const torch::Tensor &vertices, const torch::Tensor &depths, const torch::Tensor &c2w,
+                          float fx, float fy, float cx, float cy, int W, int H);
+// The faces (int32 or int64 [M,3], any device) with at least one seen vertex, in order, with faces' dtype and device ([1,3] when one face
+// is kept). A vertex id outside [0, N) raises c10::IndexError like the reference's index.
+torch::Tensor cull_mesh_faces(const torch::Tensor &faces, const torch::Tensor &seen);
 }  // namespace gssdf

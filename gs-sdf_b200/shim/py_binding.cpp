@@ -49,6 +49,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         torch::nn::Sequential decoder = make_decoder((int64_t)encoder->get_out_dim(), decoder_flat, hidden_dim, geo_num_layer);
         return gssdf::init_gs_with_sdf(*encoder, decoder, pos_W_M, map_size, bce_isigma, xyzs, mesh_res, init_opa);
     });
+    m.def("gssdf_cull_mesh_accumulate", [](torch::Tensor seen, const torch::Tensor &vertices, const torch::Tensor &depths,
+                                           const torch::Tensor &c2w, float fx, float fy, float cx, float cy, int W, int H) {
+        gssdf::cull_mesh_accumulate(seen, vertices, depths, c2w, fx, fy, cx, cy, W, H);
+    });
+    m.def("gssdf_cull_mesh_faces", &gssdf::cull_mesh_faces);
     m.def("fully_fused_projection_2dgs", &fully_fused_projection_2dgs);
     m.def("get_view_colors", [](const torch::Tensor &viewmats, const torch::Tensor &means, const torch::Tensor &radii,
                                 const torch::Tensor &colors, const torch::Tensor &camera_ids, const torch::Tensor &gaussian_ids,

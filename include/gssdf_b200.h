@@ -49,7 +49,7 @@ const char *gssdf_last_error(void);
 /* "gssdf_b200 <ver> sm_90a" */
 const char *gssdf_version(void);
 /* Argument structs grow between revisions: a binding compiled against this header must see the same number from the library. */
-#define GSSDF_ABI_REVISION 17
+#define GSSDF_ABI_REVISION 18
 int32_t gssdf_abi_revision(void);
 
 /* L2 residency hint (SURVEY 7.6): marks [ptr, ptr+bytes) as a persisting access-policy window for kernels launched on `stream` from now on
@@ -980,6 +980,56 @@ typedef struct gssdf_rot6d_to_quat_args {
     float *quaternion;            /* [n,4] */
 } gssdf_rot6d_to_quat_args;
 int gssdf_rot6d_to_quat(const gssdf_rot6d_to_quat_args *a, gssdf_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * f-7  Mesh culling against the depth images.  Replaces Mesher::cull_mesh (include/mesher/mesher.cpp:76-160), which
+ *     Mesher::save_mesh calls for mesh_culled_<prefix>.ply (:41-74). Two calls:
+ *     gssdf_mesh_cull_vertices ORs the visibility of a batch of B depth frames into a caller-owned seen[N]; frames may be streamed
+ *     in chunks of any size and order (one call over all frames equals any split). Per frame f and vertex v, in the rounding order of
+ *     the reference's CPU ATen composition (DESIGN 7h):
+ *       c  = (w2c_f @ [v,1])[:3]      each row ((w0 x + w1 y) + w2 z) + w3, every product and sum rounded on its own;  z = c.z
+ *       p  = c / |z|                  true divisions;   u = (fx p.x + 0 p.y) + cx p.z,  v = (0 p.x + fy p.y) + cy p.z (unfused)
+ *       g  = 2 (u / W) - 1, 2 (v / H) - 1                     (true divisions by the camera's W, H)
+ *       xs = (g.x + 1) ((Wd - 1) / 2), ys = (g.y + 1) ((Hd - 1) / 2)     (align_corners = true un-normalises with the IMAGE size)
+ *       d  = bilinear tap sum ((nw_val nw + ne_val ne) + sw_val sw) + se_val se with each of the last three adds one FMA; taps
+ *            outside the image read 0 (zeros padding); explicit loads, no texture filtering
+ *       seen |= 0 <= z && 0 < u < W && 0 < v < H && d + 0.02f > z
+ *     (z = 0 gives NaN through c / |z| and fails the bounds.) One thread per vertex; a vertex already seen does no work; the frame loop
+ *     stops at the first frame that sees the vertex. No host sync, no allocation. N == 0 or B == 0 is a no-op.
+ *     GSSDF_EINVAL before any launch for n outside [0, 2^31), B < 0, W, H, Hd or Wd <= 0, a row stride < Wd, or a required NULL pointer.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct gssdf_mesh_cull_vertices_args {
+    int64_t n;                    /* vertices */
+    const float *vertices;        /* [n,3] */
+    int32_t n_frames;             /* B, frames in this batch */
+    const float *w2c;             /* [B,4,4] row-major world->camera (torch.inverse of the c2w poses, computed by the caller) */
+    const float *depth;           /* frame f, row r at depth + (f * Hd + r) * depth_row_stride: [B,Hd,Wd] metres */
+    int32_t depth_h, depth_w;     /* Hd, Wd */
+    int64_t depth_row_stride;     /* floats between rows, >= Wd */
+    float fx, fy, cx, cy;
+    int32_t width, height;        /* the camera's W, H: the projection bounds and the grid normalisation */
+    uint8_t *seen;                /* [n] in / out: set to 1 where a frame sees the vertex, never cleared */
+} gssdf_mesh_cull_vertices_args;
+int gssdf_mesh_cull_vertices(const gssdf_mesh_cull_vertices_args *a, gssdf_stream_t stream);
+
+/* Stable compaction of the faces with at least one seen vertex (the reference's ~whole_mask.index({faces}).all(1), nonzero, index).
+   counts (device int32[2], overwritten): [0] kept faces, [1] error bits (1: a face index outside [0, n_vertices); that face is never
+   dereferenced and is dropped, and the caller raises ATen's index error). out has m rows, so it cannot overflow. m == 0 is a no-op that
+   still zeroes counts. GSSDF_EINVAL before any launch for m or n_vertices outside [0, 2^31), a required NULL pointer or a workspace that
+   is too small. */
+typedef struct gssdf_mesh_cull_faces_args {
+    int64_t m;                    /* faces */
+    const int32_t *faces;         /* [m,3] */
+    int64_t n_vertices;
+    const uint8_t *seen;          /* [n_vertices] */
+    int32_t *out;                 /* [m,3]: rows [0, counts[0]) are the kept faces in order */
+    int32_t *counts;              /* device int32[2] */
+    void *workspace;              /* >= gssdf_mesh_cull_workspace_bytes(m) */
+    size_t workspace_bytes;
+} gssdf_mesh_cull_faces_args;
+/* 0 for m outside [0, 2^31) */
+size_t gssdf_mesh_cull_workspace_bytes(int64_t m);
+int gssdf_mesh_cull_faces(const gssdf_mesh_cull_faces_args *a, gssdf_stream_t stream);
 
 #ifdef __cplusplus
 }
