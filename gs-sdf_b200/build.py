@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libgssdf_b200.so")
-SOURCES = ["api.cu", "project.cu", "sh.cu", "tiles.cu", "raster.cu", "sdf.cu", "sdf_tc.cu", "loss.cu", "grid_ops.cu", "optim.cu", "octree.cu", "densify.cu", "mesh.cu", "sdf_mesh.cu", "gs_init.cu", "mesh_cull.cu"]
+SOURCES = ["api.cu", "project.cu", "sh.cu", "tiles.cu", "raster.cu", "sdf.cu", "sdf_tc.cu", "loss.cu", "grid_ops.cu", "optim.cu", "octree.cu", "densify.cu", "mesh.cu", "sdf_mesh.cu", "gs_init.cu", "mesh_cull.cu", "octree_build.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
               "--extended-lambda", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
@@ -47,11 +47,11 @@ def build_shim(force=False):
     import sysconfig
 
     import torch
-    srcs = [os.path.join(HERE, "shim", f) for f in ("gsplat_cpp_shim.cpp", "tcnn_binding_shim.cpp", "cumcubes_shim.cpp", "gssdf_mesh.cpp", "gssdf_init.cpp", "py_binding.cpp")]
+    srcs = [os.path.join(HERE, "shim", f) for f in ("gsplat_cpp_shim.cpp", "tcnn_binding_shim.cpp", "cumcubes_shim.cpp", "gssdf_mesh.cpp", "gssdf_init.cpp", "gssdf_octree.cpp", "py_binding.cpp")]
     deps = srcs + [os.path.join(HERE, "shim", "include", "gsplat_cpp", h) for h in ("fully_fused_projection.h", "rasterize_to_pixels.h", "rendering.h")]
     deps.append(os.path.join(HERE, "shim", "include", "tcnn_binding", "tcnn_binding.h"))
     deps.append(os.path.join(HERE, "shim", "include", "cumcubes.hpp"))
-    deps += [os.path.join(HERE, "shim", "include", h) for h in ("gssdf_mesh.hpp", "gssdf_init.hpp", "gssdf_sdf_net.hpp")]
+    deps += [os.path.join(HERE, "shim", "include", h) for h in ("gssdf_mesh.hpp", "gssdf_init.hpp", "gssdf_sdf_net.hpp", "gssdf_octree.hpp")]
     deps.append(os.path.join(HERE, "..", "include", "gssdf_b200.h"))
     if not force and os.path.exists(SHIM_OUT) and all(os.path.getmtime(d) <= os.path.getmtime(SHIM_OUT) for d in deps):
         return SHIM_OUT

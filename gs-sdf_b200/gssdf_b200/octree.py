@@ -3,6 +3,7 @@ NeuralSLAM::sample (include/neural_mapping/neural_mapping.cpp:73-104) over the C
 data-dependent output sizes are read back ONCE per call here (the exact-shape API, like the reference's .item() calls) while
 `RaySampler` keeps everything capacity-sized on the device for the training step."""
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -17,7 +18,23 @@ def quantize_points(x, level):
     return torch.floor(torch.clamp(res * (x + 1.0) / 2.0, 0, res - 1)).to(torch.int16)
 
 
+def _host_copy(name, dev_name):
+    """A host array of the tree: set by the host build, copied from the device tensor on first use for a device-built tree."""
+    def get(self):
+        v = self.__dict__.get("_" + name)
+        if v is None:
+            v = getattr(self, dev_name).cpu().numpy()
+            self.__dict__["_" + name] = v
+        return v
+
+    def put(self, v):
+        self.__dict__["_" + name] = v
+    return property(get, put)
+
+
 class OctreeAS:
+    octree_h, exsum_h, points_h = _host_copy("octree_h", "octree_"), _host_copy("exsum_h", "prefix_"), _host_copy("points_h", "points_")
+
     def __init__(self, octree, exsum, points, pyramid, level, device, origin=(0.0, 0.0, 0.0), map_size=0.0):
         self.max_level_ = level
         self.octree_h, self.exsum_h, self.points_h, self.pyramid_ = octree, exsum, points, pyramid
@@ -45,6 +62,19 @@ class OctreeAS:
         check(lib().gssdf_octree_build_host(C.byref(a)))
         t = OctreeAS(octree, exsum, points, pyramid, level, device, origin, map_size)
         t.n_nodes = nn
+        return t
+
+    @staticmethod
+    def from_device(octree, exsum, points, pyramid, level, n_nodes, origin=(0.0, 0.0, 0.0), map_size=0.0):
+        """OctreeAS around device tensors (octree_ [max(n_nodes, 1)] uint8, prefix_ [n_nodes + 1] int32, points_ [max(n_points, 1), 3]
+        int16) and the host pyramid [2, level + 2] int32: the layout OctreeAS.from_quantized_points gives."""
+        t = OctreeAS.__new__(OctreeAS)
+        t.max_level_, t.pyramid_, t.device = level, pyramid, octree.device
+        t.octree_, t.prefix_, t.points_ = octree, exsum, points
+        t.octree_h = t.exsum_h = t.points_h = None
+        t.origin, t.map_size = tuple(float(v) for v in origin), float(map_size)
+        t.n_nodes = int(n_nodes)
+        t.ws = cabi.Workspace(octree.device)
         return t
 
     def tree_struct(self):
@@ -129,3 +159,98 @@ class RaySampler:
         a.tree = self.tree.tree_struct()
         check(lib().gssdf_sdf_sample_rays(C.byref(a), cabi._stream()))
         return self.counts
+
+
+def _f32_3(v):
+    return np.asarray(v.detach().cpu().numpy() if hasattr(v, "detach") else v, np.float32).reshape(3)
+
+
+def update_octree_as(xyz, level, origin, map_size, is_prior=False, inrange=None):
+    """SubMap::update_octree_as (sub_map.cpp:22-35) on the device: world points float32 [n,3] on a CUDA device -> OctreeAS on that device,
+    bit-identical to quantize_points(xyz_to_m1p1_pts(xyz)) -> unique -> (27-neighbour dilation + clamp unless is_prior) ->
+    OctreeAS.from_quantized_points. origin = pos_W_M, map_size = k_map_size; k_map_size_inv is 1.0f / map_size in float32.
+    inrange = (xyz_min_M, xyz_max_M): keep only the points SubMap::get_inrange_mask keeps (strictly inside the box shrunk by 1e-6), as
+    NeuralSLAM::build_occ_map does before the call. Levels 1..11 (gssdf_octree_build); the point counts are read back once, then the
+    pyramid; no other host copy is made."""
+    if not (isinstance(xyz, torch.Tensor) and xyz.is_cuda and xyz.dtype == torch.float32):
+        raise ValueError("update_octree_as: xyz must be a float32 CUDA tensor [n,3]")
+    xyz = xyz.detach().reshape(-1, 3).contiguous()
+    dev, n, f = xyz.device, xyz.shape[0], np.float32
+    pos, ms = _f32_3(origin), f(map_size)
+    a = make_args("gssdf_octree_build_device_args", n=n, xyz=xyz, origin=[float(v) for v in pos], inv_size=float(f(f(1.0) / ms)),
+                  level=level, dilate=0 if is_prior else 1)
+    if inrange is not None:  # SubMap::xyz_min_W_ = pos + xyz_min_M, get_inrange_mask: x > xyz_min_W_ + 0 + 1e-6, x < xyz_max_W_ - 0 - 1e-6
+        lo_m, hi_m = _f32_3(inrange[0]), _f32_3(inrange[1])
+        a.use_range = 1
+        a.lo = (C.c_float * 3)(*[float(f(f(pos[k] + lo_m[k]) + f(1e-6))) for k in range(3)])
+        a.hi = (C.c_float * 3)(*[float(f(f(pos[k] + hi_m[k]) - f(1e-6))) for k in range(3)])
+    nbytes = lib().gssdf_octree_build_workspace_bytes(C.c_int64(n), level)
+    if nbytes == 0:
+        check(lib().gssdf_octree_build(C.byref(a), cabi._stream()))  # raises the library's message (level out of range)
+    with torch.cuda.device(dev):
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        counts = torch.zeros(level + 2, dtype=torch.int64, device=dev)
+        a.workspace, a.workspace_bytes, a.counts = ws.data_ptr(), nbytes, counts.data_ptr()
+        st = cabi._stream()
+        check(lib().gssdf_octree_build(C.byref(a), st))
+        c = counts.tolist()
+        if c[level + 1]:
+            raise RuntimeError(f"gssdf_b200: update_octree_as: the tree has more than 2^31 - 1 points (counts {c[:level + 1]})")
+        npnt = sum(c[:level + 1])
+        nn = npnt - c[level]
+        octree = torch.empty(max(nn, 1), dtype=torch.uint8, device=dev)
+        exsum = torch.empty(nn + 1, dtype=torch.int32, device=dev)
+        points = torch.empty(max(npnt, 1), 3, dtype=torch.int16, device=dev)
+        pyramid = torch.empty(2, level + 2, dtype=torch.int32, device=dev)
+        if nn == 0:  # the host build's padding entries of an empty tree
+            octree.zero_()
+            points.zero_()
+        a.node_cap, a.point_cap = nn, npnt
+        a.octree, a.exsum, a.points, a.pyramid = octree.data_ptr(), exsum.data_ptr(), points.data_ptr(), pyramid.data_ptr()
+        check(lib().gssdf_octree_build(C.byref(a), st))
+        pyr = pyramid.cpu().numpy()
+    return OctreeAS.from_device(octree, exsum, points, pyr, level, nn, tuple(float(v) for v in pos), float(ms))
+
+
+def prior_points(tree):
+    """The points NeuralSLAM::build_occ_map writes to as_occ_prior.ply (neural_mapping.cpp:753-761): the leaf level of the point
+    hierarchy (OctreeAS::get_quantized_points), spc_ops::quantized_points_to_fpoints (spc_ops.cpp:17-25) and SubMap::m1p1_pts_to_xyz
+    (sub_map.cpp:85-90), with the same torch ops. float32 [n,3] on the tree's device."""
+    L = tree.max_level_
+    cnt, off = int(tree.pyramid_[0][L]), int(tree.pyramid_[1][L])
+    q = tree.points_[off:off + cnt]
+    r = float(np.float32(1.0 / float(1 << L)))
+    fpts = r * (2.0 * q.to(torch.float32) + 1.0) - 1.0
+    pos = torch.tensor([tree.origin], dtype=torch.float32, device=q.device)
+    return fpts * 0.5 * tree.map_size + pos
+
+
+def occ_map_frame(inner_map_size, leaf_size):
+    """The map frame of NeuralSLAM::build_occ_map (neural_mapping.cpp:706-721, params.cpp:474-478) for a given inner map size:
+    (level, map_size, xyz_min_M, xyz_max_M), float32 arithmetic as the reference's float globals."""
+    f = np.float32
+    inner, leaf = f(inner_map_size), f(leaf_size)
+    level = int(math.ceil(math.log2(float(f(f(inner + f(2 * leaf)) * f(f(1.0) / leaf))))))
+    map_size = float(f(f(2 ** level) * leaf))
+    hi = float(f(f(0.5) * inner))
+    return level, map_size, (-hi,) * 3, (hi,) * 3
+
+
+def build_occ_map(xyz, depth, min_range, max_range, inner_map_size, leaf_size):
+    """NeuralSLAM::build_occ_map (neural_mapping.cpp:683-763) from a depth point cloud: xyz float32 [..., 3] and depth [...] on a CUDA
+    device. Range filter, centre (mean) and radius (max norm) are the reference's torch ops; the inner map size shrinks to 2 * radius
+    when that is smaller; level and map size follow params.cpp. Returns (tree, frame, prior points) with frame = dict(origin, map_size,
+    level, inner_map_size, xyz_min_M, xyz_max_M)."""
+    pcl_depth = depth.reshape(-1)
+    valid = (pcl_depth > min_range) & (pcl_depth < max_range)
+    pcl = xyz.reshape(-1, 3).index_select(0, valid.nonzero().squeeze(1))
+    center = pcl.mean(0)
+    radius = np.float32((pcl - center).norm(2, 1).max().item())
+    inner = np.float32(inner_map_size)
+    if not inner < np.float32(radius * np.float32(2.0)):
+        inner = np.float32(radius * np.float32(2.0))
+    level, map_size, lo, hi = occ_map_frame(inner, leaf_size)
+    tree = update_octree_as(pcl, level, center, map_size, inrange=(lo, hi))
+    frame = dict(origin=tuple(float(v) for v in center.tolist()), map_size=map_size, level=level, inner_map_size=float(inner),
+                 xyz_min_M=lo, xyz_max_M=hi)
+    return tree, frame, prior_points(tree)

@@ -803,6 +803,44 @@ typedef struct gssdf_octree_build_args {
 } gssdf_octree_build_args;
 int gssdf_octree_build_host(gssdf_octree_build_args *a);
 
+/* SubMap::update_octree_as (include/neural_net/sub_map.cpp:22-35) on the DEVICE, from world points to the same four arrays as
+   gssdf_octree_build_host: normalise, quantise, unique, the 27-neighbour dilation + clamp (kaolin::points_to_neighbors_cuda) unless
+   dilate == 0 (the is_prior path of load_checkpoint), then kaolin's points_to_octree / octree_to_spc. Per point, with ATen's rounding
+   (one rounding per op, no contraction):
+     in range (use_range != 0):  lo[k] < x[k] < hi[k] for every k (get_inrange_mask; the caller passes hi = fl(fl(pos + max_M) - 1e-6f))
+     m = fl(fl(x - origin) * 2) * inv_size,   t = fl(res * fl(m + 1)) / 2,   q = (int16) floor(clamp(t, 0, res - 1))   (res = 2^level)
+   clamp keeps NaN and the cast turns it into 0, as ATen's CUDA cast does. Dense Morton-ordered bitmaps instead of sorting (DESIGN 7i):
+   byte i of the level-l bitmap is the child mask of level-(l-1) node i, so unique, sort and the per-level compaction are atomic ORs,
+   popcounts and one scan, and no count has to reach the host between them. Two calls with the same untouched workspace:
+     call 1 (octree == NULL) builds the bitmaps and writes counts[0..level] (points per level) and counts[level+1] (error bits);
+     call 2 (octree != NULL) only compacts into octree / exsum / points / pyramid, sized from the counts the caller read:
+       n_points = sum(counts[0..level]), n_nodes = n_points - counts[level].
+   Error bits: 1 more than 2^31 - 1 points (nothing is written by call 2); 2 call 2's node_cap or point_cap is below the counts (nothing
+   is written). No host sync, no allocation; n == 0 (or every point filtered out) is the empty tree of the host build.
+   GSSDF_EINVAL before any launch for a NULL pointer, n < 0, a level outside [1, 11] (deeper trees: OctreeAS.from_quantized_points) or
+   a negative capacity; GSSDF_ENOMEM for workspace_bytes < gssdf_octree_build_workspace_bytes(n, level). */
+typedef struct gssdf_octree_build_device_args {
+    int64_t n;                    /* points */
+    const float *xyz;             /* [n,3] world */
+    float origin[3];              /* SubMap::pos_W_M_ */
+    float inv_size;               /* k_map_size_inv */
+    int32_t level;                /* 1 .. 11 */
+    int32_t dilate;               /* 1: 27-neighbour dilation (!is_prior) */
+    int32_t use_range;            /* 1: keep only the points strictly inside (lo, hi) */
+    float lo[3], hi[3];
+    void *workspace;              /* >= gssdf_octree_build_workspace_bytes(n, level); call 2 needs call 1's contents */
+    size_t workspace_bytes;
+    int64_t *counts;              /* device int64 [level + 2] */
+    int64_t node_cap, point_cap;  /* call 2: rows allocated in octree (exsum has node_cap + 1) and points */
+    uint8_t *octree;              /* [node_cap] or NULL (call 1) */
+    int32_t *exsum;               /* [node_cap + 1] */
+    int16_t *points;              /* [point_cap,3] point hierarchy */
+    int32_t *pyramid;             /* [2, level + 2] counts | offsets (device) */
+} gssdf_octree_build_device_args;
+/* 0 for n < 0 or a level outside [1, 11]; about 2 * 8^level / 8 bytes (32 MiB at level 9, 2.3 GiB at level 11) */
+size_t gssdf_octree_build_workspace_bytes(int64_t n, int32_t level);
+int gssdf_octree_build(const gssdf_octree_build_device_args *a, gssdf_stream_t stream);
+
 /* OctreeAS::query (KW/kaolin_wisp_cpp/octree_as/octree_as.cpp:49-89 -> kaolin::query_cuda, KA/ops/spc/query_cuda.cu:26-49, identify
    KA/spc_utils.cuh:28-61) at the leaf level, and SubMap::get_valid_mask (sub_map.cpp:76-80) = pidx > -1. coords are WORLD points. */
 typedef struct gssdf_octree_query_args {
