@@ -7,6 +7,7 @@ import pytest
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
+import sdf_train_oracle as SO  # noqa: E402
 from helpers import assert_close_frac  # noqa: E402
 
 
@@ -332,7 +333,8 @@ def test_full_step_tensor_core_equals_cuda_core_path():
 def test_sdf_train_analytic_eikonal_double_backward(oracle, align_w, n):
     """eikonal_mode 1 (the reference default): eikonal + align losses on the ANALYTIC gradient d sdf/dx and their double backward
     to decoder / table, against the oracle chain (pinned to torch.autograd in tests/test_sdf_oracle.py) with tcnn's fp16
-    rounding points (dL/dy -> half x128, half corner products, half dL_ddLdy)."""
+    rounding points (dL/dy -> half x128, half corner products, half dL_ddLdy), at the 1e-3 of DESIGN section 9; and the split
+    arrangement of the training step (skip-base 7-variant forward, then V = 1 with sdf_variants) against the V = 7 call."""
     from gssdf_b200 import cabi
     dev = _dev()
     n_hidden, V, delta = 3, 7, 0.01
@@ -340,29 +342,20 @@ def test_sdf_train_analytic_eikonal_double_backward(oracle, align_w, n):
     n_params, _ = oracle.grid_setup()
     table = rng.uniform(-2e-3, 2e-3, n_params).astype(np.float32)
     mlp = _mlp(rng, 64, n_hidden)
-    x = rng.uniform(0.05, 0.95, (n, 3)).astype(np.float32)
+    # points off the knife edges of the comparison (a hidden pre-activation within 1e-4 of zero, an align-loss sign within 2e-3 |g|):
+    # there fp32-grade differences may legitimately flip a discrete choice, so they are left out rather than allowed for by a loose bound
+    P = SO.clean_points(oracle, rng, n, table, mlp, n_hidden, (0.5, 0.5, 0.5), 0.0, delta, 0.45)
+    x = P["xw"]
     gt = rng.uniform(-0.1, 0.1, n).astype(np.float32)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
     tab, half, mlp_t, xt = t(table), torch.empty(n_params, dtype=torch.float16, device=dev), t(mlp), t(x)
     cabi.sdf_table_to_half(tab, half)
     net = _tc_net(cabi, half, mlp_t, n_hidden)
     isg, bce_w, eik_w = 10.0, 1.0, 0.1
-    # ---- oracle
-    offs = np.array([[0, 0, 0], [1, 0, 0], [-1, 0, 0], [0, 1, 0], [0, -1, 0], [0, 0, 1], [0, 0, -1]], np.float32) * np.float32(delta)
-    pts = (x[None] + offs[:, None]).reshape(-1, 3).astype(np.float32)
-    r_sdf, r_y1, r_feat = oracle.sdf_fwd(pts, table, mlp, 64, n_hidden)
-    tie = _relu_ties(r_feat[:n], mlp, 64, n_hidden)  # base rows only take part in any backward
-    keep = ~tie
-    l1, v_s, v_y = oracle.sdf_losses(r_sdf, r_y1, n, 7, gt_sdf=gt, bce_isigma=isg, bce_weight=bce_w, eikonal_weight=0.0, delta=delta)
-    tg1, mg1, _ = oracle.sdf_bwd(pts, table, mlp, v_s.reshape(-1).astype(np.float32), v_y.reshape(-1).astype(np.float32), 64, n_hidden)
-    g = oracle.sdf_grad_analytic(x, table, mlp, 64, n_hidden).astype(np.float64)
-    s7 = r_sdf.reshape(7, n).astype(np.float64)
-    gnum = np.stack([s7[1] - s7[2], s7[3] - s7[4], s7[5] - s7[6]], 1) * (0.5 / delta)
-    nrm = np.linalg.norm(g, axis=1)
-    l2 = eik_w * np.mean((nrm - 1) ** 2) + align_w * np.mean(np.abs(g - gnum))
-    c = (eik_w / n) * (2 * (nrm - 1) / nrm)[:, None] * g + (align_w / (3 * n)) * np.sign(g - gnum)
-    tg2, mg2 = oracle.sdf_grad_analytic_bwd(x, table, mlp, c.astype(np.float32), 64, n_hidden)
-    # ---- GPU (ties cannot be removed from the analytic path by zeroing cotangents, so compare with a flip allowance instead)
+    # ---- oracle (tests/sdf_train_oracle.py: the oracle chains composed as the kernel composes them)
+    R = SO.compose(oracle, P, table, mlp, n_hidden, 0.0, delta, eik_w, align_w, n, gt=gt, bce_isigma=isg, bce_weight=bce_w)
+    l1, l2, mg1, mg2, tg1, tg2 = R["loss1"], R["loss2"], R["mlp1"], R["mlp2"], R["table1"], R["table2"]
+    # ---- GPU
     loss = torch.zeros(1, device=dev)
     tg, mg = torch.zeros(n_params, device=dev), torch.zeros(len(mlp), device=dev)
     cabi.sdf_train(net, xt, V, delta, t(gt), None, isg, bce_w, eik_w, 0.0, loss, tg, mg, None, eikonal_mode=1, align_weight=align_w)
@@ -375,18 +368,18 @@ def test_sdf_train_analytic_eikonal_double_backward(oracle, align_w, n):
     torch.cuda.synchronize()
     assert abs(float(loss_s) - float(loss)) <= 1e-5 * abs(float(loss))
     assert float((mg_s - mg).norm()) <= 1e-4 * float(mg.norm()) and float((tg_s - tg).norm()) <= 2e-3 * float(tg.norm())
-    assert keep.mean() > 0.98
-    assert abs(float(loss) - (l1 + l2)) <= 2e-3 * abs(l1 + l2), (float(loss), l1, l2)
+    assert abs(float(loss) - (l1 + l2)) <= 1e-4 * abs(l1 + l2), (float(loss), l1, l2)
     r_mg, r_tg = mg1 + mg2, tg1 + tg2
     mgc, tgc = mg.cpu().numpy().astype(np.float64), tg.cpu().numpy().astype(np.float64)
     assert np.linalg.norm(mg2) > 1e-3 * np.linalg.norm(mg1)  # the second-order part is a visible share of the reference gradient
     e_m, e_t = np.linalg.norm(mgc - r_mg) / np.linalg.norm(r_mg), np.linalg.norm(tgc - r_tg) / np.linalg.norm(r_tg)
-    assert e_m <= 2e-2, f"mlp grad {e_m:.2e}"
-    assert e_t <= 2e-2, f"table grad {e_t:.2e}"
     # the second-order share alone (first-order part removed with the oracle's value)
     e_m2 = np.linalg.norm((mgc - mg1) - mg2) / np.linalg.norm(mg2)
     e_t2 = np.linalg.norm((tgc - tg1) - tg2) / np.linalg.norm(tg2)
-    assert e_m2 <= 5e-2 and e_t2 <= 5e-2, (e_m2, e_t2)
+    print(f"analytic eikonal, align {align_w}: mlp {e_m:.1e} (2nd {e_m2:.1e}), table {e_t:.1e} (2nd {e_t2:.1e})")
+    assert e_m <= 1e-3, f"mlp grad {e_m:.2e}"
+    assert e_t <= 1e-3, f"table grad {e_t:.2e}"
+    assert e_m2 <= 1e-3 and e_t2 <= 1e-3, (e_m2, e_t2)
 
 
 @pytest.mark.parametrize("n,live", [(1, None), (19, None), (130, 70), (300, 0)])
