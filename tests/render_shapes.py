@@ -107,7 +107,7 @@ def two_camera_bin_sizes(tw=16, th=16, seed=1):
 # deep raster scene: a few crowded tiles of a small image
 # ------------------------------------------------------------------------------------------------------------------------------
 # (list length, opacity mode) per tile of a 128 x 64 image (8 x 4 tiles). Lengths: every sort tier, one list beyond the shared-memory
-# sort, k*256 and k*256 +- 1 (forward / default backward batch), k*192 +- 1 (the 192-splat backward variant).
+# sort, and k*128, k*128 +- 1 (forward stages of 128 splats; every k*128 is also a k*64 edge of the backward's 64-splat stages).
 # low: opacity 1.2..2 / 255 -- whole lists are composited (no pixel saturates); high: 0.3..0.95 -- pixels saturate within a few
 # dozen splats, so last_ids stops early and the backward starts mid-batch; mixed: low in front, high behind the 60 % depth quantile.
 RASTER_W, RASTER_H = 128, 64
@@ -127,14 +127,15 @@ def screen_splat_transforms(means2d, depths, sigma, tilt):
     """Ray transforms [n,3,3] of splats facing the camera at pixel scale `sigma`, centred on means2d, with depth d at the centre and a
     depth slope tilt * d per unit of the splat's local (u, v): rows are the x, y and z rows of the splat-to-screen homography, i.e. a
     local point (u, v) maps to the homogeneous pixel u * U + v * V + W with U = (s d + cx a, cy a, a), V = (cx b, s d + cy b, b),
-    W = (cx d, cy d, d), (a, b) = tilt * d."""
+    W = (cx d, cy d, d), (a, b) = tilt * d. `sigma` [n] is isotropic; [n, 2] gives separate x and y scales."""
     m = np.asarray(means2d, np.float64)
     d = np.asarray(depths, np.float64)
     s = np.asarray(sigma, np.float64)
+    sx, sy = (s[:, 0], s[:, 1]) if s.ndim == 2 else (s, s)
     a, b = tilt[:, 0] * d, tilt[:, 1] * d
     cx, cy = m[:, 0], m[:, 1]
-    U = np.stack([s * d + cx * a, cy * a, a], 1)
-    V = np.stack([cx * b, s * d + cy * b, b], 1)
+    U = np.stack([sx * d + cx * a, cy * a, a], 1)
+    V = np.stack([cx * b, sy * d + cy * b, b], 1)
     Wv = np.stack([cx * d, cy * d, d], 1)
     return np.ascontiguousarray(np.stack([U, V, Wv], 2).astype(np.float32))  # [n, row(x,y,z), col(U,V,W)]
 
@@ -199,10 +200,10 @@ def deep_raster_scene(seed=0, zero_rows=0.1):
 
 
 def lengths_of_interest(lengths):
-    """the designed list lengths that sit on a batch boundary of the forward / backward (256) or the backward variant (192)."""
+    """the designed list lengths that sit on a stage edge of the forward (128 splats) or the backward (64 splats)."""
     L = [int(x) for x in lengths]
     near = lambda q: sorted({x for x in L if x >= q - 1 and (x % q in (0, 1, q - 1))})
-    return dict(k256=near(256), k192=near(192))
+    return dict(k128=near(128), k64=near(64))
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

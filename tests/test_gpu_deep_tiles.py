@@ -5,13 +5,9 @@
   against the oracle;
 * culled tile lists on the bit-mask path (cap <= isect_cap) and the per-tile path (cap > isect_cap);
 * the capacity-overflow contract (flagged, clamped, never written past isect_cap) through tile encode, raster and SplatRenderer;
-* raster forward / backward over lists up to 30000 deep, on and around the 256 / 192 batch boundaries, against the fp64 oracle, with the
-  mirror API, with the trainer's arguments and with the 192-splat backward variant.
+* raster forward / backward over lists up to 30000 deep, on and around the forward's 128-splat and the backward's 64-splat stage edges,
+  against the fp64 oracle, with the mirror API and with the trainer's arguments.
 The inputs come from tests/render_shapes.py (checked on the host by test_render_shapes_host.py)."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -27,7 +23,6 @@ from gssdf_b200 import scene as S  # noqa: E402
 SENT32 = -0x2152411   # guard-tail sentinels
 SENT64 = -0x21524110DEAD
 SENT_F = -1234.5
-VARIANT_ENV = "GSSDF_RASTER_BWD_VARIANT"
 
 
 def _dev():
@@ -77,44 +72,50 @@ def _conics(dev, sc):
 
 
 class _Raster:
-    """raster2dgs_fwd / bwd through the C ABI on one scene, with a workspace sized for the backward so that reuse_fwd can share it."""
+    """raster2dgs_fwd / bwd through the C ABI on one scene (sc["C"] cameras, optional sc["backgrounds"]), with a workspace sized for the
+    backward so that reuse_fwd can share it."""
 
     def __init__(self, dev, sc, isect_cap, guard=0):
         from gssdf_b200 import cabi
         self.dev, self.sc, self.isect_cap, self.guard = dev, sc, int(isect_cap), guard
         self.nnz = len(sc["depths"])
+        self.C = int(sc.get("C", 1))
         self.ws = cabi.Workspace(dev)
-        self.ws.get(cabi.lib().gssdf_raster2dgs_bwd_workspace_bytes(1, sc["W"], sc["H"], self.nnz, cabi._lib.C.c_int64(self.isect_cap)))
+        self.ws.get(cabi.lib().gssdf_raster2dgs_bwd_workspace_bytes(self.C, sc["W"], sc["H"], self.nnz, cabi._lib.C.c_int64(self.isect_cap)))
         self.inp = {k: _t(sc[k], dev) for k in ("means2d", "ray_transforms", "colors", "opacities", "normals")}
+        bg = sc.get("backgrounds")
+        self.bg = None if bg is None else _t(bg, dev)
 
     def fwd(self, counts, off, flat, distort=True):
         from gssdf_b200 import cabi
-        W, H, dev = self.sc["W"], self.sc["H"], self.dev
+        W, H, C, dev = self.sc["W"], self.sc["H"], self.C, self.dev
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
-        out = dict(render_colors=z(1, H, W, 3), render_depths=z(1, H, W, 1), render_alphas=z(1, H, W, 1), render_normals=z(1, H, W, 3),
-                   render_median=z(1, H, W, 1), last_ids=z(1, H, W, dt=torch.int32), median_ids=z(1, H, W, dt=torch.int32),
+        out = dict(render_colors=z(C, H, W, 3), render_depths=z(C, H, W, 1), render_alphas=z(C, H, W, 1), render_normals=z(C, H, W, 3),
+                   render_median=z(C, H, W, 1), last_ids=z(C, H, W, dt=torch.int32), median_ids=z(C, H, W, dt=torch.int32),
                    visibilities=z(self.nnz, 1))
         if distort:
-            out.update(render_distort=z(1, H, W, 1), render_Ts=z(1, H, W, 2))
+            out.update(render_distort=z(C, H, W, 1), render_Ts=z(C, H, W, 2))
         i = self.inp
-        cabi.raster2dgs_fwd(1, W, H, 16, 3, self.nnz, counts, i["means2d"], i["ray_transforms"], i["colors"], i["opacities"], i["normals"],
-                            None, off, flat, out, self.ws, isect_cap=self.isect_cap)
+        cabi.raster2dgs_fwd(C, W, H, 16, 3, self.nnz, counts, i["means2d"], i["ray_transforms"], i["colors"], i["opacities"], i["normals"],
+                            self.bg, off, flat, out, self.ws, isect_cap=self.isect_cap)
         torch.cuda.synchronize()
         return out
 
-    def bwd(self, counts, off, flat, state, ct, reuse_fwd):
+    def bwd(self, counts, off, flat, state, ct, reuse_fwd, absgrad=False):
         from gssdf_b200 import cabi
         dev, n, G = self.dev, self.nnz, self.guard
         f = lambda *s: torch.full(s, SENT_F, dtype=torch.float32, device=dev)
         g = dict(v_means2d=f(n + G, 2), v_ray_transforms=f(n + G, 3, 3), v_colors=f(n + G, 3), v_opacities=f(n + G), v_normals=f(n + G, 3),
                  v_densify=f(n + G, 2))
+        if absgrad:
+            g["v_means2d_abs"] = f(n + G, 2)
         s = {k: (v if torch.is_tensor(v) else _t(v, dev)) for k, v in state.items()}
         c = {k: _t(v, dev) for k, v in ct.items()}
         i = self.inp
-        cabi.raster2dgs_bwd(1, self.sc["W"], self.sc["H"], 16, 3, n, counts, i["means2d"], i["ray_transforms"], i["colors"], i["opacities"],
-                            i["normals"], None, off, flat, s["render_alphas"], s.get("render_Ts"), s["last_ids"], s["median_ids"],
-                            c["v_render_colors"], c["v_render_depths"], c["v_render_alphas"], c["v_render_normals"], c["v_render_median"], g,
-                            self.ws, isect_cap=self.isect_cap, reuse_fwd=reuse_fwd)
+        cabi.raster2dgs_bwd(self.C, self.sc["W"], self.sc["H"], 16, 3, n, counts, i["means2d"], i["ray_transforms"], i["colors"],
+                            i["opacities"], i["normals"], self.bg, off, flat, s["render_alphas"], s.get("render_Ts"), s["last_ids"],
+                            s["median_ids"], c["v_render_colors"], c["v_render_depths"], c["v_render_alphas"], c["v_render_normals"],
+                            c["v_render_median"], g, self.ws, isect_cap=self.isect_cap, reuse_fwd=reuse_fwd)
         torch.cuda.synchronize()
         return {k: _np(v) for k, v in g.items()}
 
@@ -346,7 +347,8 @@ def test_splat_renderer_reports_isect_overflow():
 # ------------------------------------------------------------------------------------------------------------------------------
 def _print_lists(sc):
     li = lengths_of_interest(sc["list_len"])
-    print(f"raster lists: {sorted(int(x) for x in sc['list_len'] if x)}; on 256-batch edges {li['k256']}; on 192-batch edges {li['k192']}")
+    print(f"raster lists: {sorted(int(x) for x in sc['list_len'] if x)}; on 128-splat forward stage edges {li['k128']}; "
+          f"on 64-splat backward stage edges {li['k64']}")
 
 
 def test_raster_deep_lists_mirror_api(deep):
@@ -386,22 +388,4 @@ def _trainer_config(deep, label):
 
 
 def test_raster_deep_lists_trainer_config(deep):
-    if os.environ.get(VARIANT_ENV, "0") not in ("", "0"):
-        pytest.skip(f"{VARIANT_ENV} is set: this process runs the backward variant")
     _trainer_config(deep, "trainer")
-
-
-def test_raster_deep_lists_trainer_config_bwd_variant_192(deep):
-    """(c) = (b) with the 192-splat backward stages (GSSDF_RASTER_BWD_VARIANT=1), in a fresh process since the library reads the knob
-    once per process."""
-    if os.environ.get(VARIANT_ENV) == "1":
-        _trainer_config(deep, "variant 1")
-        return
-    _dev()
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    node = f"{os.path.abspath(__file__)}::test_raster_deep_lists_trainer_config_bwd_variant_192"
-    py = [sys.executable] + (["-s"] if sys.flags.no_user_site else [])
-    r = subprocess.run(py + ["-m", "pytest", "-q", "-p", "no:cacheprovider", "-rA", node], cwd=root, env={**os.environ, VARIANT_ENV: "1"},
-                       capture_output=True, text=True, timeout=1200)
-    print(r.stdout[-3000:])
-    assert r.returncode == 0 and "1 passed" in r.stdout, r.stdout[-3000:] + r.stderr[-2000:]

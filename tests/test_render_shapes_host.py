@@ -47,11 +47,10 @@ def test_deep_raster_builder(oracle):
     h = tier_histogram(L)
     assert h["global_sort"] >= 1 and h["tier3"] >= 2 and h["tier2"] >= 1 and h["tier1"] >= 1 and h["tier0"] >= 1
     li = lengths_of_interest(L)
-    print(f"lists {sorted(int(x) for x in L)}; 256-batch edges {li['k256']}; 192-batch edges {li['k192']}")
-    for q in (256, 192):
+    print(f"lists {sorted(int(x) for x in L)}; 128-splat forward stage edges {li['k128']}; 64-splat backward stage edges {li['k64']}")
+    for q in (128, 64):
         have = set(li[f"k{q}"])
-        assert any(x % q == 0 for x in have) or q == 192
-        assert any(x % q == 1 for x in have) and any(x % q == q - 1 for x in have)
+        assert any(x % q == 0 for x in have) and any(x % q == 1 for x in have) and any(x % q == q - 1 for x in have)
         assert len(have) >= 6
     # un-culled (reference) lists: the designed ones plus the decoys' entries in neighbouring tiles
     sizes, _, _ = _oracle_sizes(oracle, sc, 1, tw, th)
