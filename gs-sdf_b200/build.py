@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libgssdf_b200.so")
-SOURCES = ["api.cu", "project.cu", "sh.cu", "tiles.cu", "raster.cu", "sdf.cu", "sdf_tc.cu", "loss.cu", "grid_ops.cu", "optim.cu", "octree.cu", "densify.cu", "mesh.cu", "sdf_mesh.cu", "gs_init.cu", "mesh_cull.cu", "octree_build.cu"]
+SOURCES = ["api.cu", "project.cu", "sh.cu", "tiles.cu", "raster.cu", "sdf.cu", "sdf_tc.cu", "loss.cu", "grid_ops.cu", "optim.cu", "octree.cu", "densify.cu", "mesh.cu", "sdf_mesh.cu", "gs_init.cu", "mesh_cull.cu", "octree_build.cu", "mesh_eval.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
               "--extended-lambda", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 

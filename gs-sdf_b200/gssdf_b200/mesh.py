@@ -194,3 +194,157 @@ def cull_mesh(vertices, faces, depths, c2w, K, W, H, chunk=None, seen=None):
         bad = f[(f < 0) | (f >= n)][0]
         raise IndexError(f"index {int(bad)} is out of bounds for dimension 0 with size {n}")
     return v, out[:kept], seen
+
+
+# ---- f-9 structure metrics (DESIGN 7j) ----------------------------------------------------------------------------------------------
+METRIC_KEYS = ("MAE_accuracy (cm)", "MAE_completeness (cm)", "Chamfer_L1 (cm)", "Chamfer_L2 (cm)", "Precision [Accuracy] (%)",
+               "Recall [Completeness] (%)", "F-score (%)", "Spacing (cm)", "Inlier_threshold (cm)", "Outlier_truncation_acc (cm)",
+               "Outlier_truncation_com (cm)")
+
+
+def gt_bounding_box(points):
+    """open3d's get_minimal_oriented_bounding_box rule on the host: for each triangle of the convex hull and each of its edges, the
+    hull's axis-aligned box in the frame (the edge, the triangle's normal x the edge, the normal); the box of smallest volume wins.
+    points: [n,3] array or tensor (n >= 4, not coplanar). Returns (center [3], R [3,3] whose columns are the axes, extent [3]) in fp64."""
+    from scipy.spatial import ConvexHull
+    p = np.asarray(points.detach().cpu() if hasattr(points, "detach") else points, np.float64).reshape(-1, 3)
+    hull = ConvexHull(p)
+    hp = p[hull.vertices]
+    best = None
+    for tri in hull.simplices:
+        v = p[tri]
+        n = np.cross(v[1] - v[0], v[2] - v[0])
+        if not np.linalg.norm(n) > 0:
+            continue
+        n = n / np.linalg.norm(n)
+        for e in range(3):  # each edge of the triangle as the first axis: the result does not depend on the hull's vertex order
+            u = v[(e + 1) % 3] - v[e]
+            u = u / np.linalg.norm(u)
+            R = np.stack([u, np.cross(n, u), n], 1)
+            loc = hp @ R
+            lo, hi = loc.min(0), loc.max(0)
+            vol = float(np.prod(hi - lo))
+            if best is None or vol < best[0]:
+                best = (vol, R @ ((lo + hi) * 0.5), R, hi - lo)
+    if best is None:
+        raise ValueError("gssdf_b200: gt_bounding_box needs a cloud that spans three dimensions")
+    return best[1], best[2], best[3]
+
+
+def sample_surface(vertices, faces, n_samples, samples, counts, ws, seed=0, box=None):
+    """Raw gssdf_mesh_sample_uniform: crop by box (center, R, extent) if given, then n_samples area-uniform samples into samples (CUDA
+    float64 [n_samples,3], face order); counts (CUDA int32 [2]) gets [samples written, error bits]."""
+    m = faces.shape[0]
+    w = ws.get(lib().gssdf_mesh_sample_uniform_workspace_bytes(m))
+    kw = dict(use_box=0)
+    if box is not None:
+        c, R, e = (np.asarray(x, np.float64) for x in box)
+        kw = dict(use_box=1, box_center=c.tolist(), box_R=R.reshape(-1).tolist(), box_extent=e.tolist())
+    a = make_args("gssdf_mesh_sample_uniform_args", n_vertices=vertices.shape[0], vertices=vertices, m=m, faces=faces,
+                  n_samples=int(n_samples), seed=int(seed), samples=samples, counts=counts, workspace=w, workspace_bytes=w.numel(), **kw)
+    check(lib().gssdf_mesh_sample_uniform(C.byref(a), cabi._stream()))
+
+
+def voxel_down_sample(points, voxel_size, out_points, out_keys, origin, counts, ws, n_live=None):
+    """Raw gssdf_voxel_downsample: voxel means of points (CUDA float32 / float64 [cap,3]; rows [0, min(cap, *n_live)) when n_live, a
+    CUDA int32 tensor, is given) into out_points (float64 [cap,3]) / out_keys (int64 [cap]) in Morton order; origin (float64 [3]) gets
+    the grid's min bound, counts (int32 [2]) [voxels, error bits]."""
+    if points.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"gssdf_b200: points must be float32 or float64, got {points.dtype}")
+    cap = points.shape[0]
+    w = ws.get(lib().gssdf_voxel_downsample_workspace_bytes(cap))
+    a = make_args("gssdf_voxel_downsample_args", cap=cap, points=points, dtype=int(points.dtype == torch.float64), n_live=n_live,
+                  voxel_size=float(voxel_size), out_points=out_points, out_keys=out_keys, origin=origin, counts=counts, workspace=w,
+                  workspace_bytes=w.numel())
+    check(lib().gssdf_voxel_downsample(C.byref(a), cabi._stream()))
+
+
+def nn_distances(queries, targets, target_keys, target_origin, voxel_size, trunc, threshold, clamp_beyond, result, ws, n_queries=None,
+                 n_targets=None, distances=None, cell_shift=3):
+    """Raw gssdf_nn_truncated: the truncated nearest neighbour of each query (float64 [cap,3]) among the targets (a voxel_down_sample
+    output with the same voxel_size); result (a 40-byte CUDA buffer) gets gssdf_nn_result, distances (float64 [cap], optional) the
+    per-query distance (+inf when dropped, trunc when clamped)."""
+    cap = queries.shape[0]
+    w = ws.get(lib().gssdf_nn_truncated_workspace_bytes(cap))
+    a = make_args("gssdf_nn_truncated_args", cap_queries=cap, queries=queries, n_queries=n_queries, cap_targets=targets.shape[0],
+                  targets=targets, target_keys=target_keys, n_targets=n_targets, target_origin=target_origin, voxel_size=float(voxel_size),
+                  cell_shift=int(cell_shift), trunc=float(trunc), threshold=float(threshold), clamp_beyond=int(bool(clamp_beyond)),
+                  distances=distances, result=result, workspace=w, workspace_bytes=w.numel())
+    check(lib().gssdf_nn_truncated(C.byref(a), cabi._stream()))
+
+
+def nn_result(buf):
+    """(n_kept, n_inliers, n_clamped, sum_d, sum_d2) from the 40 bytes of a gssdf_nn_result (numpy uint8 or a tensor)."""
+    b = np.ascontiguousarray(buf.cpu().numpy() if hasattr(buf, "cpu") else buf, np.uint8)
+    i, d = b[:24].view(np.int64), b[24:40].view(np.float64)
+    return int(i[0]), int(i[1]), int(i[2]), float(d[0]), float(d[1])
+
+
+def _metrics(n_pred, n_gt, acc, com, down_sample_res, threshold, truncation_acc, truncation_com):
+    """eval_utils.eval_mesh's dictionary from the two results (kept, inliers, clamped, sum d, sum d^2; the sums skip clamped queries). Either side empty gives empty lists on both
+    sides, as nn_correspondance does; an empty mean is NaN, and F-score is NaN when precision and recall are both 0."""
+    nan = float("nan")
+    if n_pred == 0 or n_gt == 0:
+        acc = com = (0, 0, 0, 0.0, 0.0)
+    mean = lambda s, n: s / n if n else nan
+    # a clamped query adds exactly trunc: an all-clamped side averages to exactly trunc
+    dp = mean(acc[3], acc[0]) + truncation_acc * mean(float(acc[2]), acc[0])
+    dr = mean(com[3], com[0]) + truncation_com * mean(float(com[2]), com[0])
+    dp2 = mean(acc[4], acc[0]) + truncation_acc * truncation_acc * mean(float(acc[2]), acc[0])
+    dr2 = mean(com[4], com[0]) + truncation_com * truncation_com * mean(float(com[2]), com[0])
+    prec, rec = mean(float(acc[1]), acc[0]) * 100.0, mean(float(com[1]), com[0]) * 100.0
+    f = 2 * prec * rec / (prec + rec) if (prec + rec) != 0 else nan
+    vals = (dp * 100.0, dr * 100.0, 0.5 * (dp + dr) * 100.0, math.sqrt(0.5 * (dp2 + dr2)) * 100.0, prec, rec, f, down_sample_res * 100.0,
+            threshold * 100.0, truncation_acc * 100.0, truncation_com * 100.0)
+    return dict(zip(METRIC_KEYS, vals))
+
+
+def eval_mesh(vertices, faces, gt_points, down_sample_res=0.01, threshold=0.02, truncation_acc=0.2, truncation_com=0.2, gt_bbx_mask_on=True,
+              mesh_sample_point=10_000_000, seed=0, box=None, cell_shift=3):
+    """eval_utils.eval_mesh (evaluator.py's defaults) on the GPU (DESIGN 7j). vertices: CUDA float32 [V,3]; faces: CUDA int32 [F,3];
+    gt_points: float32 / float64 [G,3] (moved to the mesh's device). The prediction is cropped by `box` (center, R, extent), by default
+    gt_bounding_box(gt_points) -- a host computation that depends only on the dataset, so callers scoring several meshes pass it once --
+    then sampled, both clouds down-sampled, and scored with truncated nearest neighbours both ways. One asynchronous sequence with one
+    read-back. Returns the reference's 11-key dict (cm and %). A face index outside [0, V) raises ATen's IndexError."""
+    v = cabi._req(vertices, torch.float32, "vertices")
+    f = cabi._req(faces, torch.int32, "faces")
+    if v.dim() != 2 or v.shape[1] != 3 or f.dim() != 2 or f.shape[1] != 3:
+        raise ValueError(f"gssdf_b200: vertices and faces must be [N,3] and [M,3], got {tuple(v.shape)} and {tuple(f.shape)}")
+    if not down_sample_res > 0:
+        raise ValueError(f"gssdf_b200: down_sample_res must be positive, got {down_sample_res}")
+    dev = v.device
+    g = torch.as_tensor(gt_points).to(dev)
+    if g.dtype not in (torch.float32, torch.float64) or g.dim() != 2 or g.shape[1] != 3:
+        raise ValueError(f"gssdf_b200: gt_points must be float32 or float64 [G,3], got {g.dtype} {tuple(g.shape)}")
+    g = g.contiguous()
+    if gt_bbx_mask_on and box is None:
+        box = gt_bounding_box(g)
+    N, G = int(mesh_sample_point), g.shape[0]
+    ws = cabi.Workspace(dev)
+    ws.get(max(lib().gssdf_mesh_sample_uniform_workspace_bytes(f.shape[0]), lib().gssdf_voxel_downsample_workspace_bytes(max(N, G)),
+               lib().gssdf_nn_truncated_workspace_bytes(max(N, G))))
+    # one device buffer for everything read back: int32 counts of the three stages, then the two gssdf_nn_result records
+    state = torch.zeros(112, dtype=torch.uint8, device=dev)
+    c32 = state[:32].view(torch.int32)  # [0:2] samples, [2:4] predicted voxels, [4:6] ground-truth voxels
+    res_acc, res_com = state[32:72], state[72:112]
+    samples = torch.empty(max(N, 1), 3, dtype=torch.float64, device=dev)
+    sample_surface(v, f, N, samples, c32[0:2], ws, seed=seed, box=box if gt_bbx_mask_on else None)
+    pred = torch.empty(max(N, 1), 3, dtype=torch.float64, device=dev)
+    pred_keys = torch.empty(max(N, 1), dtype=torch.int64, device=dev)
+    gt = torch.empty(max(G, 1), 3, dtype=torch.float64, device=dev)
+    gt_keys = torch.empty(max(G, 1), dtype=torch.int64, device=dev)
+    origins = torch.empty(2, 3, dtype=torch.float64, device=dev)
+    voxel_down_sample(samples[:N], down_sample_res, pred, pred_keys, origins[0], c32[2:4], ws, n_live=c32[0:1])
+    voxel_down_sample(g, down_sample_res, gt, gt_keys, origins[1], c32[4:6], ws)
+    nn_distances(pred[:N], gt[:G], gt_keys[:G], origins[1], down_sample_res, truncation_acc, threshold, False, res_acc, ws,
+                 n_queries=c32[2:3], n_targets=c32[4:5], cell_shift=cell_shift)
+    nn_distances(gt[:G], pred[:N], pred_keys[:N], origins[0], down_sample_res, truncation_com, threshold, True, res_com, ws,
+                 n_queries=c32[4:5], n_targets=c32[2:3], cell_shift=cell_shift)
+    h = state.cpu().numpy()
+    c = h[:32].view(np.int32)
+    if c[1] & 1:
+        bad = f[(f < 0) | (f >= v.shape[0])][0]
+        raise IndexError(f"index {int(bad)} is out of bounds for dimension 0 with size {v.shape[0]}")
+    if (c[3] | c[5]) & 1:
+        raise RuntimeError(f"gssdf_b200: voxel_size {down_sample_res} is too small for the cloud's range (more than 2^21 voxels per axis)")
+    return _metrics(int(c[2]), int(c[4]), nn_result(h[32:72]), nn_result(h[72:112]), down_sample_res, threshold, truncation_acc, truncation_com)

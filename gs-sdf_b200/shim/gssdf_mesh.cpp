@@ -7,6 +7,7 @@
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 
+#include <algorithm>
 #include <cmath>
 #include <stdexcept>
 
@@ -202,4 +203,99 @@ torch::Tensor gssdf::cull_mesh_faces(const torch::Tensor &faces, const torch::Te
     const int32_t *cn = h.data_ptr<int32_t>();
     if (cn[1] & 1) bad_index(f);
     return out.slice(0, 0, cn[0]).to(faces.device(), faces.scalar_type());
+}
+
+std::map<std::string, double> gssdf::eval_mesh(const torch::Tensor &vertices, const torch::Tensor &faces, const torch::Tensor &gt_points,
+                                               const torch::Tensor &box, double down_sample_res, double threshold, double truncation_acc,
+                                               double truncation_com, bool gt_bbx_mask_on, int64_t mesh_sample_point, int64_t seed) {
+    torch::NoGradGuard no_grad;
+    TORCH_CHECK(vertices.dim() == 2 && vertices.size(1) == 3 && faces.dim() == 2 && faces.size(1) == 3, "vertices and faces must be [N,3], [M,3]");
+    TORCH_CHECK(gt_points.dim() == 2 && gt_points.size(1) == 3, "gt_points must be [G,3]");
+    TORCH_CHECK(!gt_bbx_mask_on || box.numel() == 15, "box must hold center[3], R[9] (row-major, columns = axes), extent[3]");
+    TORCH_CHECK(down_sample_res > 0, "down_sample_res must be positive");
+    const auto dev = vertices.is_cuda() ? vertices.device() : torch::Device(torch::kCUDA, c10::cuda::current_device());
+    const c10::cuda::CUDAGuard guard(dev);
+    auto stream = reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream());
+    const auto opt = torch::TensorOptions().device(dev);
+    const int64_t nv = vertices.size(0);
+    if (faces.scalar_type() == torch::kLong && faces.numel() && ((faces < 0) | (faces >= nv)).any().item<bool>()) {
+        const int64_t bad = faces.masked_select((faces < 0) | (faces >= nv)).flatten()[0].item<int64_t>();
+        TORCH_CHECK_INDEX(false, "index ", bad, " is out of bounds for dimension 0 with size ", nv);
+    }
+    torch::Tensor v = vertices.to(opt.dtype(torch::kFloat)).contiguous();
+    torch::Tensor f = faces.to(opt.dtype(torch::kInt)).contiguous();
+    torch::Tensor g = gt_points.to(dev, gt_points.scalar_type() == torch::kDouble ? torch::kDouble : torch::kFloat).contiguous();
+    const int64_t N = mesh_sample_point, G = g.size(0);
+    const size_t ws_bytes = std::max({gssdf_mesh_sample_uniform_workspace_bytes(f.size(0)),
+                                      gssdf_voxel_downsample_workspace_bytes(std::max(N, G)), gssdf_nn_truncated_workspace_bytes(std::max(N, G))});
+    torch::Tensor ws = torch::empty({(int64_t)std::max<size_t>(ws_bytes, 1)}, opt.dtype(torch::kByte));
+    // one device buffer for everything read back: int32 counts of the three stages, then the two gssdf_nn_result records
+    torch::Tensor state = torch::zeros({32 + 2 * (int64_t)sizeof(gssdf_nn_result)}, opt.dtype(torch::kByte));
+    auto *c32 = reinterpret_cast<int32_t *>(state.data_ptr<uint8_t>());
+    auto *res = reinterpret_cast<gssdf_nn_result *>(state.data_ptr<uint8_t>() + 32);
+    torch::Tensor samples = torch::empty({std::max<int64_t>(N, 1), 3}, opt.dtype(torch::kDouble));
+    torch::Tensor pred = torch::empty({std::max<int64_t>(N, 1), 3}, opt.dtype(torch::kDouble));
+    torch::Tensor pred_keys = torch::empty({std::max<int64_t>(N, 1)}, opt.dtype(torch::kLong));
+    torch::Tensor gt = torch::empty({std::max<int64_t>(G, 1), 3}, opt.dtype(torch::kDouble));
+    torch::Tensor gt_keys = torch::empty({std::max<int64_t>(G, 1)}, opt.dtype(torch::kLong));
+    torch::Tensor origins = torch::empty({2, 3}, opt.dtype(torch::kDouble));
+
+    gssdf_mesh_sample_uniform_args s{};
+    s.n_vertices = nv, s.vertices = v.data_ptr<float>(), s.m = f.size(0), s.faces = f.data_ptr<int32_t>();
+    if (gt_bbx_mask_on) {
+        torch::Tensor b = box.to(torch::kCPU, torch::kDouble).contiguous();
+        const double *bp = b.data_ptr<double>();
+        s.use_box = 1;
+        for (int k = 0; k < 3; ++k) s.box_center[k] = bp[k], s.box_extent[k] = bp[12 + k];
+        for (int k = 0; k < 9; ++k) s.box_R[k] = bp[3 + k];
+    }
+    s.n_samples = N, s.seed = seed, s.samples = samples.data_ptr<double>(), s.counts = c32;
+    s.workspace = ws.data_ptr(), s.workspace_bytes = (size_t)ws.numel();
+    check(gssdf_mesh_sample_uniform(&s, stream));
+    auto down = [&](int64_t cap, const void *pts, int dtype, const int32_t *n_live, torch::Tensor &out, torch::Tensor &keys, double *origin,
+                    int32_t *counts) {
+        gssdf_voxel_downsample_args a{};
+        a.cap = cap, a.points = pts, a.dtype = dtype, a.n_live = n_live, a.voxel_size = down_sample_res;
+        a.out_points = out.data_ptr<double>(), a.out_keys = keys.data_ptr<int64_t>(), a.origin = origin, a.counts = counts;
+        a.workspace = ws.data_ptr(), a.workspace_bytes = (size_t)ws.numel();
+        check(gssdf_voxel_downsample(&a, stream));
+    };
+    down(N, samples.data_ptr(), 1, c32, pred, pred_keys, origins.data_ptr<double>(), c32 + 2);
+    down(G, g.data_ptr(), g.scalar_type() == torch::kDouble ? 1 : 0, nullptr, gt, gt_keys, origins.data_ptr<double>() + 3, c32 + 4);
+    auto nn = [&](int64_t cq, const torch::Tensor &q, const int32_t *nq, int64_t ct, const torch::Tensor &t, const torch::Tensor &tk,
+                  const double *origin, const int32_t *nt, double trunc, int clamp, gssdf_nn_result *r) {
+        gssdf_nn_truncated_args a{};
+        a.cap_queries = cq, a.queries = q.data_ptr<double>(), a.n_queries = nq;
+        a.cap_targets = ct, a.targets = t.data_ptr<double>(), a.target_keys = tk.data_ptr<int64_t>(), a.n_targets = nt;
+        a.target_origin = origin, a.voxel_size = down_sample_res, a.cell_shift = 3;  // cells of 8 voxels per axis: the fastest of 1-3 on the box room (DESIGN 7j)
+        a.trunc = trunc, a.threshold = threshold, a.clamp_beyond = clamp, a.result = r;
+        a.workspace = ws.data_ptr(), a.workspace_bytes = (size_t)ws.numel();
+        check(gssdf_nn_truncated(&a, stream));
+    };
+    nn(N, pred, c32 + 2, G, gt, gt_keys, origins.data_ptr<double>() + 3, c32 + 4, truncation_acc, 0, res);
+    nn(G, gt, c32 + 4, N, pred, pred_keys, origins.data_ptr<double>(), c32 + 2, truncation_com, 1, res + 1);
+
+    torch::Tensor h = state.cpu();
+    const auto *hc = reinterpret_cast<const int32_t *>(h.data_ptr<uint8_t>());
+    const auto *hr = reinterpret_cast<const gssdf_nn_result *>(h.data_ptr<uint8_t>() + 32);
+    if (hc[1] & 1) {
+        const int64_t bad = f.masked_select((f < 0) | (f >= nv)).flatten()[0].item<int64_t>();
+        TORCH_CHECK_INDEX(false, "index ", bad, " is out of bounds for dimension 0 with size ", nv);
+    }
+    TORCH_CHECK(!((hc[3] | hc[5]) & 1), "gssdf_b200: voxel_size ", down_sample_res, " is too small for the cloud's range");
+    // eval_utils.eval_mesh's dictionary (gssdf_b200.mesh._metrics): either side empty empties both lists; an empty mean is NaN
+    const double nan = std::nan("");
+    gssdf_nn_result acc = hr[0], com = hr[1];
+    if (hc[2] == 0 || hc[4] == 0) acc = com = gssdf_nn_result{};
+    auto mean = [&](double s_, int64_t n) { return n ? s_ / (double)n : nan; };
+    const double dp = mean(acc.sum_d, acc.n_kept) + truncation_acc * mean((double)acc.n_clamped, acc.n_kept);
+    const double dr = mean(com.sum_d, com.n_kept) + truncation_com * mean((double)com.n_clamped, com.n_kept);
+    const double dp2 = mean(acc.sum_d2, acc.n_kept) + truncation_acc * truncation_acc * mean((double)acc.n_clamped, acc.n_kept);
+    const double dr2 = mean(com.sum_d2, com.n_kept) + truncation_com * truncation_com * mean((double)com.n_clamped, com.n_kept);
+    const double prec = mean((double)acc.n_inliers, acc.n_kept) * 100.0, rec = mean((double)com.n_inliers, com.n_kept) * 100.0;
+    const double fs = (prec + rec) != 0 ? 2 * prec * rec / (prec + rec) : nan;
+    return {{"MAE_accuracy (cm)", dp * 100.0}, {"MAE_completeness (cm)", dr * 100.0}, {"Chamfer_L1 (cm)", 0.5 * (dp + dr) * 100.0},
+            {"Chamfer_L2 (cm)", std::sqrt(0.5 * (dp2 + dr2)) * 100.0}, {"Precision [Accuracy] (%)", prec}, {"Recall [Completeness] (%)", rec},
+            {"F-score (%)", fs}, {"Spacing (cm)", down_sample_res * 100.0}, {"Inlier_threshold (cm)", threshold * 100.0},
+            {"Outlier_truncation_acc (cm)", truncation_acc * 100.0}, {"Outlier_truncation_com (cm)", truncation_com * 100.0}};
 }

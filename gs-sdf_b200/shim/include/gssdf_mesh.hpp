@@ -4,6 +4,8 @@
 #pragma once
 #include <torch/torch.h>
 
+#include <map>
+#include <string>
 #include <vector>
 
 #include "tcnn_binding/tcnn_binding.h"
@@ -31,4 +33,15 @@ void cull_mesh_accumulate(torch::Tensor &seen, const torch::Tensor &vertices, co
 // The faces (int32 or int64 [M,3], any device) with at least one seen vertex, in order, with faces' dtype and device ([1,3] when one face
 // is kept). A vertex id outside [0, N) raises c10::IndexError like the reference's index.
 torch::Tensor cull_mesh_faces(const torch::Tensor &faces, const torch::Tensor &seen);
+
+// eval_utils.eval_mesh, which NeuralSLAM::eval_mesh (include/neural_mapping/neural_mapping.cpp:1404-1433) runs through evaluator.py, in
+// process (gssdf_mesh_sample_uniform / gssdf_voxel_downsample / gssdf_nn_truncated; DESIGN 7j, INTEGRATION 3g). vertices [V,3] and
+// faces [F,3] (int32 or int64) of mesh_culled_<res>.ply and the ground-truth cloud gt_points [G,3] (float32 or float64), on the CPU or
+// the GPU; box: center[3], R[9] (row-major, columns = axes), extent[3] as 15 doubles (gssdf_b200.mesh.gt_bounding_box of the ground
+// truth; ignored when gt_bbx_mask_on is false). Returns the reference's 11 metrics (cm, %) with its key names, the same values as
+// gssdf_b200.mesh.eval_mesh; one read-back. A face index outside [0, V) raises c10::IndexError.
+std::map<std::string, double> eval_mesh(const torch::Tensor &vertices, const torch::Tensor &faces, const torch::Tensor &gt_points,
+                                        const torch::Tensor &box, double down_sample_res = 0.01, double threshold = 0.02,
+                                        double truncation_acc = 0.2, double truncation_com = 0.2, bool gt_bbx_mask_on = true,
+                                        int64_t mesh_sample_point = 10000000, int64_t seed = 0);
 }  // namespace gssdf

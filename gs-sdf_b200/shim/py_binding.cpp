@@ -55,6 +55,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         gssdf::cull_mesh_accumulate(seen, vertices, depths, c2w, fx, fy, cx, cy, W, H);
     });
     m.def("gssdf_cull_mesh_faces", &gssdf::cull_mesh_faces);
+    m.def("gssdf_eval_mesh", &gssdf::eval_mesh);
     m.def("gssdf_update_octree_as", &gssdf::update_octree_as);
     m.def("fully_fused_projection_2dgs", &fully_fused_projection_2dgs);
     m.def("get_view_colors", [](const torch::Tensor &viewmats, const torch::Tensor &means, const torch::Tensor &radii,

@@ -1069,6 +1069,111 @@ typedef struct gssdf_mesh_cull_faces_args {
 size_t gssdf_mesh_cull_workspace_bytes(int64_t m);
 int gssdf_mesh_cull_faces(const gssdf_mesh_cull_faces_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-9  Structure metrics of an exported mesh.  Replaces eval_utils.eval_mesh, which NeuralSLAM::eval_mesh
+ *     (include/neural_mapping/neural_mapping.cpp:1404-1433) runs through eval/structure_metrics/evaluator.py on mesh_culled_<res>.ply:
+ *     crop, uniform surface sampling, voxel down-sampling of both clouds, truncated nearest neighbours both ways (DESIGN 7j). Three calls
+ *     whose counts chain on the device (sampler counts[0] -> down-sampler n_live -> nearest-neighbour n_queries / n_targets), so a whole
+ *     evaluation is one asynchronous sequence with one read-back at the end. None of them allocates or syncs; all arguments are checked
+ *     before the first launch; every `_rn` below is one IEEE rounding (no contraction). Empty inputs are no-ops that still zero counts.
+ * ------------------------------------------------------------------------------------------ */
+/* Crop + SamplePointsUniformly. Per face t (vertex ids outside [0, n_vertices) set error bit 1: the face is never dereferenced and gets
+   no samples, and the caller raises ATen's index error):
+     kept  = no box, or all three vertices inside the box: |((d0 R0i + d1 R1i) + d2 R2i)| <= extent_i * 0.5 for i = 0..2, d = v - center
+     area  = kept ? 0.5 * sqrt((c0^2 + c1^2) + c2^2) : 0,   c = (v0 - v1) x (v0 - v2)  (fp64, vertices widened from fp32)
+     P     = inclusive prefix sum of area in fp64, S = P[m-1]; fixed association (tiles of 2048 faces, 8 per thread summed in order,
+             tile offsets in order), so identical from run to run; it differs from a sequential sum in the last bits
+     end_t = round(fl(P_t / S) * N) (half away from zero; 0 for every face when S == 0), so face t owns samples [end_{t-1}, end_t)
+   Sample i of face t with ordinal j = i - end_{t-1}: (x0, x1, x2, x3) = Philox-4x32-10(counter (j, t, 0, 0), key (seed & 0xffffffff,
+   seed >> 32)); r1 = ((x0 >> 5) * 2^26 + (x1 >> 6)) * 2^-53, r2 likewise from (x2, x3); s = sqrt(r1), a = 1 - s, b = s * (1 - r2),
+   c = s * r2; p = (a v0 + b v1) + c v2 per coordinate. Samples are in face order. counts (device int32[2], overwritten): [0] samples
+   written (N when some kept face has area, else 0; feed it to gssdf_voxel_downsample's n_live), [1] error bits.
+   GSSDF_EINVAL before any launch for m, n_vertices or n_samples outside [0, 2^31), a negative box extent, a required NULL pointer or a
+   workspace that is too small. */
+typedef struct gssdf_mesh_sample_uniform_args {
+    int64_t n_vertices;
+    const float *vertices;        /* [n_vertices,3] */
+    int64_t m;                    /* faces */
+    const int32_t *faces;         /* [m,3] */
+    int32_t use_box;              /* 1: crop by the oriented box below (gt_bbx_mask_on) */
+    double box_center[3];
+    double box_R[9];              /* row-major 3x3; column i is box axis i */
+    double box_extent[3];         /* full side lengths along the axes */
+    int64_t n_samples;            /* N */
+    int64_t seed;
+    double *samples;              /* [N,3] */
+    int32_t *counts;              /* device int32[2] */
+    void *workspace;              /* >= gssdf_mesh_sample_uniform_workspace_bytes(m) */
+    size_t workspace_bytes;
+} gssdf_mesh_sample_uniform_args;
+/* 0 for m outside [0, 2^31) */
+size_t gssdf_mesh_sample_uniform_workspace_bytes(int64_t m);
+int gssdf_mesh_sample_uniform(const gssdf_mesh_sample_uniform_args *a, gssdf_stream_t stream);
+
+/* VoxelDownSample. The cloud is rows [0, n) of points, n = min(cap, *n_live) (n = cap when n_live is NULL):
+     origin = min over the cloud (per axis, fp64) - voxel_size * 0.5
+     voxel  = floor((p - origin) / voxel_size) per axis (fp64 true division), packed into a 63-bit Morton key (21 bits per axis)
+     mean   = the voxel's points summed sequentially in fp64 in index order (a stable sort keeps it), / count (true division)
+   Outputs are in Morton order: out_points / out_keys rows [0, counts[0]). Rows n .. cap - 1 get a sentinel key that sorts last, so no
+   count has to reach the host. counts (device int32[2], overwritten): [0] voxels, [1] error bits (1: a voxel index outside [0, 2^21) on
+   some axis -- a range of more than 2^21 voxels or a non-finite coordinate; the outputs are then meaningless and the caller raises).
+   GSSDF_EINVAL before any launch for cap outside [0, 2^31 - 1), a dtype other than 0 / 1, voxel_size <= 0 or non-finite, a required NULL
+   pointer or a workspace that is too small. */
+typedef struct gssdf_voxel_downsample_args {
+    int64_t cap;                  /* rows of points and of every output */
+    const void *points;           /* [cap,3] */
+    int32_t dtype;                /* 0: float32, 1: float64 */
+    const int32_t *n_live;        /* device int32 or NULL */
+    double voxel_size;
+    double *out_points;           /* [cap,3] voxel means */
+    int64_t *out_keys;            /* [cap] Morton keys of the voxels, ascending */
+    double *origin;               /* device double[3] */
+    int32_t *counts;              /* device int32[2] */
+    void *workspace;              /* >= gssdf_voxel_downsample_workspace_bytes(cap) */
+    size_t workspace_bytes;
+} gssdf_voxel_downsample_args;
+/* 0 for cap outside [0, 2^31 - 1) */
+size_t gssdf_voxel_downsample_workspace_bytes(int64_t cap);
+int gssdf_voxel_downsample(const gssdf_voxel_downsample_args *a, gssdf_stream_t stream);
+
+/* Truncated nearest neighbour of each query among the targets, which must be a gssdf_voxel_downsample output (points, keys, origin,
+   counts[0] as n_targets) with the same voxel_size. Targets are grouped into cells of voxel_size * 2^cell_shift by key >> 3 cell_shift
+   (no second sort); one thread per query searches ring by ring and stops when the best squared distance is at most the squared
+   distance to the unvisited cells (less a slack of 1e-9 cells) or when that bound reaches trunc. Squared distances are
+   ((dx dx + dy dy) + dz dz)_rn, d = sqrt_rn. Query i is kept when d^2 < trunc^2 (trunc^2 = trunc * trunc in fp64); otherwise it is
+   dropped (clamp_beyond == 0, distances[i] = +inf) or kept at d = trunc (clamp_beyond == 1). With no targets every query is beyond.
+   result (device, overwritten): kept queries, inliers (kept with d < threshold), clamped queries, and the sums of d and of fl(d * d)
+   over the kept queries that were not clamped (a clamped query adds trunc, so the mean is sum_d / n_kept + trunc * n_clamped / n_kept,
+   exactly trunc when every query is clamped); fixed block trees and a fixed final order, no atomics: bit-identical from run to run for
+   a given cap_queries.
+   GSSDF_EINVAL before any launch for a cap outside [0, 2^31), voxel_size <= 0 or non-finite, cell_shift outside [0, 20], trunc <= 0 or
+   non-finite, a NaN threshold, trunc / (voxel_size * 2^cell_shift) > 1024, a required NULL pointer or a workspace that is too small. */
+typedef struct gssdf_nn_result {
+    int64_t n_kept, n_inliers, n_clamped;
+    double sum_d, sum_d2;
+} gssdf_nn_result;
+typedef struct gssdf_nn_truncated_args {
+    int64_t cap_queries;
+    const double *queries;        /* [cap_queries,3] */
+    const int32_t *n_queries;     /* device int32 or NULL (cap_queries) */
+    int64_t cap_targets;
+    const double *targets;        /* [cap_targets,3], Morton order */
+    const int64_t *target_keys;   /* [cap_targets] */
+    const int32_t *n_targets;     /* device int32 or NULL (cap_targets) */
+    const double *target_origin;  /* device double[3]: the targets' down-sampling origin */
+    double voxel_size;            /* the targets' voxel size */
+    int32_t cell_shift;
+    double trunc, threshold;
+    int32_t clamp_beyond;
+    double *distances;            /* [cap_queries] or NULL */
+    gssdf_nn_result *result;      /* device */
+    void *workspace;              /* >= gssdf_nn_truncated_workspace_bytes(cap_queries) */
+    size_t workspace_bytes;
+} gssdf_nn_truncated_args;
+/* 0 for cap_queries outside [0, 2^31) */
+size_t gssdf_nn_truncated_workspace_bytes(int64_t cap_queries);
+int gssdf_nn_truncated(const gssdf_nn_truncated_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
