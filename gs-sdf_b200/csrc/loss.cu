@@ -27,6 +27,16 @@ struct SsimWindow {
     float w[kWin];
 };
 
+// The loss w (1 - mean S) is a small difference of two large terms (0.036 of 0.2 at 1080p), so the per-warp sums of S meet in one
+// double (atomic adds of ~10^4 partials into a float drifted by ~1e-5 of the loss, in an order-dependent way); the last warp to add
+// its partial writes w - w / N * sum into the float loss with a single rounding.
+struct SsimSum {
+    double *sum;       // workspace tail, zeroed before the launch
+    unsigned *done;    // warps that have added their partial
+    unsigned n_warps;  // warps that add one (x0 < W)
+    double scale;      // w / N
+};
+
 static SsimWindow make_window() {  // loss_utils.cpp:6-14 (float tensor, normalised by its sum)
     SsimWindow g;
     const float sigma = 1.5f;
@@ -42,7 +52,7 @@ static SsimWindow make_window() {  // loss_utils.cpp:6-14 (float tensor, normali
 
 // grid (strips / kSsimWarps, bands, C * 3); band_h rows per band
 __global__ void __launch_bounds__(kSsimWarps * 32)
-dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__restrict__ maps, float scale_loss, int band_h) {
+dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__restrict__ maps, const SsimSum red, int band_h) {
     __shared__ float s_row[kSsimWarps][2][2][kRowW + 2];  // [warp][buffer][x | y][column]
     const int W = a.image_width, H = a.image_height;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -71,7 +81,7 @@ dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__r
     for (int k = 0; k < kWin; ++k)
 #pragma unroll
         for (int q = 0; q < 5; ++q) acc[k][q] = 0.f;
-    float part = 0.f;
+    double part = 0.0;
     float xa, ya, xb, yb;
     fetch(y0 - kHalf, xa, ya, xb, yb);
     const int n_in = (y1 - y0) + 2 * kHalf;  // input rows y0 - 5 .. y1 + 4
@@ -119,11 +129,16 @@ dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__r
             }
         }
     }
-    part = warp_sum(part);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
     if (lane == 0) {
-        float s = -scale_loss * part;                                                         // - w / N * sum S
-        if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && warp == 0) s += a.w_dssim;  // + w * 1
-        atomicAdd(a.loss_out, s);
+        atomicAdd(red.sum, part);
+        __threadfence();
+        if (atomicAdd(red.done, 1u) == red.n_warps - 1) {  // every other partial is in
+            __threadfence();
+            const double total = atomicAdd(red.sum, 0.0);
+            atomicAdd(a.loss_out, (float)((double)a.w_dssim - red.scale * total));  // w * 1 - w / N * sum S
+        }
     }
 }
 
@@ -209,9 +224,12 @@ dssim_bwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, const floa
 
 using namespace gssdf;
 
+// three derivative maps [3][C*3][H][W], then the loss reduction's double sum and warp counter (16-byte aligned tail)
+static size_t dssim_tail_offset(int32_t C, int32_t W, int32_t H) { return ((size_t)9 * C * W * H * sizeof(float) + 15) / 16 * 16; }
+
 extern "C" size_t gssdf_dssim_workspace_bytes(int32_t C, int32_t W, int32_t H) {
     if (C <= 0 || W <= 0 || H <= 0) return 0;
-    return (size_t)9 * C * W * H * sizeof(float);
+    return dssim_tail_offset(C, W, H) + 16;
 }
 
 // rows per band: a warp marches (band + 10) row steps and the launch takes ceil(CTAs / resident CTAs) rounds of them (the kernels
@@ -248,7 +266,12 @@ extern "C" int gssdf_dssim_loss(const gssdf_dssim_loss_args *a, gssdf_stream_t s
     const int gx = cdiv(cdiv(a->image_width, kStrip), kSsimWarps);
     {
         const int band = ssim_band_height((const void *)dssim_fwd_kernel, a->image_width, a->image_height, a->C);
-        dssim_fwd_kernel<<<dim3(gx, cdiv(a->image_height, band), a->C * 3), kSsimWarps * 32, 0, st>>>(*a, win, maps, (float)(a->w_dssim / n), band);
+        const dim3 grid(gx, cdiv(a->image_height, band), a->C * 3);
+        char *tail = reinterpret_cast<char *>(a->workspace) + dssim_tail_offset(a->C, a->image_width, a->image_height);
+        SsimSum red{reinterpret_cast<double *>(tail), reinterpret_cast<unsigned *>(tail + 8),
+                    (unsigned)cdiv(a->image_width, kStrip) * grid.y * grid.z, (double)a->w_dssim / n};
+        GSSDF_CUDA_OK(cudaMemsetAsync(tail, 0, 16, st));
+        dssim_fwd_kernel<<<grid, kSsimWarps * 32, 0, st>>>(*a, win, maps, red, band);
         GSSDF_LAUNCH_OK("dssim_fwd_kernel");
     }
     if (a->v_out_colors) {

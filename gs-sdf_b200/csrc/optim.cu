@@ -9,35 +9,75 @@
 // Here: one sweep. Algorithmic bytes per parameter = 4 (p) + 4 (g) + 4 (m) + 4 (v) read, 4 + 4 + 4 + 4 written (g is zeroed in the same
 // pass = zero_grad) + 2 for the fp16 shadow of table entries: 32 B (34 B) -> 74.3 M parameters at 1 M splats / SH 3 = 2.4 GB, an
 // HBM-bound streaming kernel (128-bit loads/stores, grid = whole chunks of 4096 parameters).
+//
+// Row groups (the trainer's features_dc / features_rest, 65 % of those bytes) are updated lazily: only the rows a step's camera sees
+// have a gradient, so the same launch visits just those rows (replaying the zero-gradient steps each missed, then applying step t) and
+// a sweep over every row runs once per GSSDF_ADAM_WINDOW steps (DESIGN.md section 7c).
 #include <cuda_fp16.h>
 
+#include "adam.cuh"
 #include "common.cuh"
 
 namespace gssdf {
 
 constexpr int kAdamThreads = 256, kAdamPerThread = 4, kAdamChunk = kAdamThreads * kAdamPerThread * 4;  // 4096 parameters per CTA
+constexpr int kAdamRowsPerCta = 64;  // row groups: 64 rows x (3 + 45) parameters at SH degree 3 = 12 per thread
 
 struct AdamPlan {
-    int32_t first_block[GSSDF_ADAM_MAX_GROUPS + 1];  // CTA range of each group
+    int32_t first_block[GSSDF_ADAM_MAX_GROUPS + 1];  // CTA range of each dense group
+    int8_t dense[GSSDF_ADAM_MAX_GROUPS];             // args.groups index of dense group i
+    int8_t rowg[GSSDF_ADAM_MAX_ROW_GROUPS];          // args.groups index of row group k
+    int32_t n_dense, n_rowg, row_width;              // row_width = summed widths of the row groups
+    int64_t n_rows;                                  // rows of every row group
     float step_size[GSSDF_ADAM_MAX_GROUPS];          // lr / (1 - beta1^t)
     float inv_sqrt_bc2;                              // 1 / sqrt(1 - beta2^t)
 };
 
-__device__ __forceinline__ void adam_one(float &p, float &g, float &m, float &v, float b1, float b2, float eps, float gs, float step_size,
-                                         float isb2) {
-    const float gr = g * gs;
-    m = b1 * m + (1.f - b1) * gr;
-    v = b2 * v + (1.f - b2) * gr * gr;
-    const float denom = sqrtf(v) * isb2 + eps;
-    p -= step_size * (m / denom);
+// Rows [blk * kAdamRowsPerCta, +kAdamRowsPerCta) of the visit list; a row's parameters are consecutive threads, the row groups side by
+// side. Every thread of a row reads the row's stamp before the CTA barrier; one thread per row writes the new stamp after it.
+__device__ __forceinline__ void adam_rows(const gssdf_adam_args &a, const AdamPlan &plan, const gssdf_adam_replay &r, int64_t blk) {
+    const int64_t n = a.row_ids ? min((int64_t)a.row_count->nnz, (int64_t)a.row_cap) : plan.n_rows;
+    const int64_t k0 = blk * kAdamRowsPerCta;
+    if (k0 >= n) return;  // CTA-uniform
+    const int t = a.step, rw = plan.row_width, w0 = a.groups[plan.rowg[0]].row_width;
+    const float b1 = a.beta1, b2 = a.beta2, eps = a.eps, gs = a.grad_scale;
+    for (int e = threadIdx.x; e < kAdamRowsPerCta * rw; e += kAdamThreads) {
+        const int kr = e / rw, c = e - kr * rw;
+        const int64_t k = k0 + kr;
+        if (k >= n) break;
+        const int64_t row = a.row_ids ? a.row_ids[k] : k;
+        const int gk = (plan.n_rowg > 1 && c >= w0) ? 1 : 0;
+        const gssdf_adam_group grp = a.groups[plan.rowg[gk]];
+        const int64_t i = grp.offset + row * grp.row_width + (c - (gk ? w0 : 0));
+        float p = a.params[i], m = a.exp_avg[i], v = a.exp_avg_sq[i];
+        const int from = r.last[row];
+        if (a.replay_only) {
+            adam_replay(p, m, v, from, t, r, gk);
+        } else {
+            adam_replay(p, m, v, from, t - 1, r, gk);
+            adam_one(p, a.grads[i], m, v, b1, b2, eps, gs, plan.step_size[plan.rowg[gk]], plan.inv_sqrt_bc2);
+            if (a.zero_grads) a.grads[i] = 0.f;
+        }
+        a.params[i] = p; a.exp_avg[i] = m; a.exp_avg_sq[i] = v;
+    }
+    __syncthreads();
+    for (int kr = threadIdx.x; kr < kAdamRowsPerCta; kr += kAdamThreads) {
+        const int64_t k = k0 + kr;
+        if (k < n) r.last[a.row_ids ? a.row_ids[k] : k] = t;
+    }
 }
 
-__global__ void __launch_bounds__(kAdamThreads) adam_kernel(const gssdf_adam_args a, const AdamPlan plan) {
-    int gi = 0;
+__global__ void __launch_bounds__(kAdamThreads) adam_kernel(const gssdf_adam_args a, const AdamPlan plan, const gssdf_adam_replay r) {
+    if ((int)blockIdx.x >= plan.first_block[plan.n_dense]) {
+        adam_rows(a, plan, r, (int64_t)blockIdx.x - plan.first_block[plan.n_dense]);
+        return;
+    }
+    int di = 0;
 #pragma unroll 1
-    while (gi + 1 < a.n_groups && (int)blockIdx.x >= plan.first_block[gi + 1]) ++gi;
+    while (di + 1 < plan.n_dense && (int)blockIdx.x >= plan.first_block[di + 1]) ++di;
+    const int gi = plan.dense[di];
     const gssdf_adam_group grp = a.groups[gi];
-    const int64_t chunk0 = (int64_t)(blockIdx.x - plan.first_block[gi]) * kAdamChunk;
+    const int64_t chunk0 = (int64_t)(blockIdx.x - plan.first_block[di]) * kAdamChunk;
     const float b1 = a.beta1, b2 = a.beta2, eps = a.eps, gs = a.grad_scale, ss = plan.step_size[gi], isb2 = plan.inv_sqrt_bc2;
     float *P = a.params + grp.offset, *G = a.grads + grp.offset, *M = a.exp_avg + grp.offset, *V = a.exp_avg_sq + grp.offset;
     __half *Hs = (grp.half_shadow && a.table_half) ? reinterpret_cast<__half *>(a.table_half) : nullptr;
@@ -66,8 +106,8 @@ __global__ void __launch_bounds__(kAdamThreads) adam_kernel(const gssdf_adam_arg
             }
         } else {
             for (int64_t k = e; k < min(e + 4, grp.count); ++k) {
-                float p = P[k], g = G[k], m = M[k], v = V[k];
-                adam_one(p, g, m, v, b1, b2, eps, gs, ss, isb2);
+                float p = P[k], m = M[k], v = V[k];
+                adam_one(p, G[k], m, v, b1, b2, eps, gs, ss, isb2);
                 P[k] = p; M[k] = m; V[k] = v;
                 if (a.zero_grads) G[k] = 0.f;
                 if (Hs) Hs[k] = __float2half_rn(p);
@@ -110,6 +150,27 @@ using namespace gssdf;
 
 extern "C" int gssdf_sdf_mlp_pack(const gssdf_sdf_net *net, void *packed, gssdf_stream_t stream);
 
+// The per-step scalars, in double and rounded once: the replays of a step must use the bits its dense update would have used.
+static void adam_bias_corrections(float beta1, float beta2, int step, double &bc1, double &bc2) {
+    bc1 = 1.0 - std::pow((double)beta1, (double)step);
+    bc2 = 1.0 - std::pow((double)beta2, (double)step);
+}
+static float adam_step_size(float lr, double bc1) { return (float)((double)lr / bc1); }
+static float adam_inv_sqrt_bc2(double bc2) { return (float)(1.0 / std::sqrt(bc2)); }
+
+extern "C" int gssdf_adam_replay_push(gssdf_adam_replay *r, int32_t step, float lr0, float lr1) {
+    GSSDF_REQUIRE(r != nullptr && step >= 1, GSSDF_EINVAL, "adam_replay_push: null replay or step < 1");
+    GSSDF_REQUIRE(r->beta1 >= 0.f && r->beta1 < 1.f && r->beta2 >= 0.f && r->beta2 < 1.f, GSSDF_EINVAL, "adam_replay_push: bad betas");
+    double bc1, bc2;
+    adam_bias_corrections(r->beta1, r->beta2, step, bc1, bc2);
+    const int w = step & (GSSDF_ADAM_WINDOW - 1);
+    r->step = step;
+    r->step_size[w] = adam_step_size(lr0, bc1);
+    r->step_size[GSSDF_ADAM_WINDOW + w] = adam_step_size(lr1, bc1);
+    r->inv_sqrt_bc2[w] = adam_inv_sqrt_bc2(bc2);
+    return GSSDF_OK;
+}
+
 extern "C" int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "adam_step: null args");
     GSSDF_REQUIRE(a->params && a->grads && a->exp_avg && a->exp_avg_sq, GSSDF_EINVAL, "adam_step: null buffer");
@@ -118,20 +179,44 @@ extern "C" int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream) 
     GSSDF_REQUIRE(a->beta1 >= 0.f && a->beta1 < 1.f && a->beta2 >= 0.f && a->beta2 < 1.f && a->eps >= 0.f, GSSDF_EINVAL, "adam_step: bad betas / eps");
     AdamPlan plan{};
     int64_t blocks = 0;
-    const double bc1 = 1.0 - std::pow((double)a->beta1, (double)a->step), bc2 = 1.0 - std::pow((double)a->beta2, (double)a->step);
+    double bc1, bc2;
+    adam_bias_corrections(a->beta1, a->beta2, a->step, bc1, bc2);
+    plan.n_rows = -1;
     for (int gi = 0; gi < a->n_groups; ++gi) {
         const gssdf_adam_group &g = a->groups[gi];
-        GSSDF_REQUIRE(g.offset >= 0 && g.count >= 0, GSSDF_EINVAL, "adam_step: bad group %d", gi);
+        GSSDF_REQUIRE(g.offset >= 0 && g.count >= 0 && g.row_width >= 0, GSSDF_EINVAL, "adam_step: bad group %d", gi);
         GSSDF_REQUIRE(!g.half_shadow || a->table_half, GSSDF_EINVAL, "adam_step: group %d wants a half shadow but table_half is null", gi);
-        plan.first_block[gi] = (int32_t)blocks;
-        plan.step_size[gi] = (float)((double)g.lr / bc1);
+        plan.step_size[gi] = adam_step_size(g.lr, bc1);
+        if (g.row_width > 0) {
+            GSSDF_REQUIRE(plan.n_rowg < GSSDF_ADAM_MAX_ROW_GROUPS && !g.half_shadow && g.count % g.row_width == 0, GSSDF_EINVAL,
+                          "adam_step: bad row group %d", gi);
+            GSSDF_REQUIRE(plan.n_rows < 0 || plan.n_rows == g.count / g.row_width, GSSDF_EINVAL, "adam_step: row groups differ in rows");
+            plan.n_rows = g.count / g.row_width;
+            plan.row_width += g.row_width;
+            plan.rowg[plan.n_rowg++] = (int8_t)gi;
+            continue;
+        }
+        if (a->replay_only) continue;
+        plan.first_block[plan.n_dense] = (int32_t)blocks;
+        plan.dense[plan.n_dense++] = (int8_t)gi;
         blocks += (g.count + kAdamChunk - 1) / kAdamChunk;
         GSSDF_REQUIRE(blocks < (int64_t)1 << 31, GSSDF_EINVAL, "adam_step: too many parameters for one launch");
     }
-    plan.first_block[a->n_groups] = (int32_t)blocks;
-    plan.inv_sqrt_bc2 = (float)(1.0 / std::sqrt(bc2));
+    plan.first_block[plan.n_dense] = (int32_t)blocks;
+    plan.inv_sqrt_bc2 = adam_inv_sqrt_bc2(bc2);
+    gssdf_adam_replay r{};
+    if (plan.n_rowg > 0 && plan.n_rows > 0) {
+        GSSDF_REQUIRE(a->replay && a->replay->last && a->replay->step == a->step, GSSDF_EINVAL, "adam_step: row groups need replay (step %d)", a->step);
+        GSSDF_REQUIRE(a->replay->beta1 == a->beta1 && a->replay->beta2 == a->beta2 && a->replay->eps == a->eps && a->grad_scale > 0.f,
+                      GSSDF_EINVAL, "adam_step: replay constants differ from the step's, or grad_scale <= 0");
+        GSSDF_REQUIRE(!a->row_ids || (a->row_count && a->row_cap >= 0), GSSDF_EINVAL, "adam_step: row_ids without row_count / row_cap");
+        r = *a->replay;
+        const int64_t visit = a->row_ids ? std::min<int64_t>(a->row_cap, plan.n_rows) : plan.n_rows;  // grid for capacity, exit on the count
+        blocks += (visit + kAdamRowsPerCta - 1) / kAdamRowsPerCta;
+        GSSDF_REQUIRE(blocks < (int64_t)1 << 31, GSSDF_EINVAL, "adam_step: too many parameters for one launch");
+    }
     if (blocks > 0) {
-        adam_kernel<<<(unsigned)blocks, kAdamThreads, 0, (cudaStream_t)stream>>>(*a, plan);
+        adam_kernel<<<(unsigned)blocks, kAdamThreads, 0, (cudaStream_t)stream>>>(*a, plan, r);
         GSSDF_LAUNCH_OK("adam_kernel");
     }
     if (a->net && a->mlp_packed) return gssdf_sdf_mlp_pack(a->net, a->mlp_packed, stream);

@@ -304,15 +304,41 @@ def isotropic_loss(N, cap, counts, gaussian_ids, scales, raw_params, weight, los
     check(lib().gssdf_isotropic_loss(_lib.C.byref(a), _stream()))
 
 
+ADAM_WINDOW = 64  # GSSDF_ADAM_WINDOW
+
+
+class AdamReplay:
+    """Host half of the lazy row groups (gssdf_adam_replay): the device stamps `last` [rows] (int32) and the scalars of the last
+    ADAM_WINDOW steps. push(t, lr0, lr1) once per step, before that step's adam_step."""
+
+    def __init__(self, last, beta1=0.9, beta2=0.999, eps=1e-15):
+        self.last = last
+        self.s = make_args("gssdf_adam_replay", last=last, beta1=beta1, beta2=beta2, eps=eps)
+
+    def push(self, step, lr0, lr1):
+        check(lib().gssdf_adam_replay_push(_lib.C.byref(self.s), int(step), float(lr0), float(lr1)))
+
+    @property
+    def step(self):
+        return self.s.step
+
+    def ptr(self):
+        return _lib.C.addressof(self.s)
+
+
 def adam_step(params, grads, exp_avg, exp_avg_sq, groups, step, beta1=0.9, beta2=0.999, eps=1e-15, grad_scale=1.0, zero_grads=True,
-              table_half=None, net=None, mlp_packed=None):
-    """groups: list of (offset, count, lr, half_shadow). `net` (gssdf_sdf_net struct, kept alive by the caller) + mlp_packed: re-pack the
-    decoder's bf16 operand image after the update."""
+              table_half=None, net=None, mlp_packed=None, replay=None, row_ids=None, row_count=None, row_cap=0, replay_only=False):
+    """groups: list of (offset, count, lr, half_shadow[, row_width]). `net` (gssdf_sdf_net struct, kept alive by the caller) + mlp_packed:
+    re-pack the decoder's bf16 operand image after the update. Row groups (row_width > 0) need `replay` (AdamReplay, pushed for `step`);
+    row_ids + row_count (device counts, ->nnz) + row_cap: visit those rows only, else every row (see gssdf_adam_args)."""
     a = make_args("gssdf_adam_args", params=params, grads=grads, exp_avg=exp_avg, exp_avg_sq=exp_avg_sq, n_groups=len(groups), step=step,
                   beta1=beta1, beta2=beta2, eps=eps, grad_scale=grad_scale, zero_grads=int(bool(zero_grads)), table_half=table_half,
-                  mlp_packed=mlp_packed)
-    for i, (off, cnt, lr, hs) in enumerate(groups):
+                  mlp_packed=mlp_packed, replay=replay.ptr() if replay is not None else None, row_ids=row_ids, row_count=row_count,
+                  row_cap=int(row_cap), replay_only=int(bool(replay_only)))
+    for i, grp in enumerate(groups):
+        off, cnt, lr, hs = grp[:4]
         a.groups[i].offset, a.groups[i].count, a.groups[i].lr, a.groups[i].half_shadow = int(off), int(cnt), float(lr), int(bool(hs))
+        a.groups[i].row_width = int(grp[4]) if len(grp) > 4 else 0
     if net is not None:
         a.net = _lib.C.cast(_lib.C.pointer(net), _lib.C.c_void_p)
     check(lib().gssdf_adam_step(_lib.C.byref(a), _stream()))

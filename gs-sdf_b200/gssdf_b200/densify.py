@@ -75,6 +75,7 @@ class Densifier:
         for k in ("params", "exp_avg", "exp_avg_sq"):  # the SDF segment (hash table + decoder) travels with the buffer swap
             self.alt[k][t0:].copy_(old[k][t0:])
         T.params, T.exp_avg, T.exp_avg_sq, T.anchors_buf = self.alt["params"], self.alt["exp_avg"], self.alt["exp_avg_sq"], self.alt["anchors"]
+        T.stamp_sh_current()  # reading T.params above brought every SH row current: the remapped rows are copies of current rows
         self.alt = old
         self.state, self.state2 = self.state2, self.state
         T.set_live(n_new)

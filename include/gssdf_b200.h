@@ -152,6 +152,24 @@ int gssdf_project2dgs_bwd(const gssdf_project2dgs_bwd_args *a, gssdf_stream_t st
  *     GSF/csrc/SphericalHarmonicsCUDA.cu:374-399) with mask min(radii)>0; clamp_min(c+0.5, 0).
  *     The [nnz,K,3] gathers the reference materialises are fused away.
  * ------------------------------------------------------------------------------------------ */
+/* Lazy Adam over row groups. A zero-gradient Adam step still moves a parameter (m and v decay), so a row whose gradient is zero may
+   skip its steps and have them REPLAYED, bit for bit, when it is next read: last[r] is the step at which row r (of every row group)
+   was last brought current, and bringing it to step t runs the arithmetic of the dense update with g = +0 for the steps
+   last[r]+1 .. t. The per-step scalars of the last GSSDF_ADAM_WINDOW steps travel by value; step s lives in slot s % WINDOW, so every
+   row must be within WINDOW - 1 steps of the current one (the caller sweeps every row at least once per window). */
+#define GSSDF_ADAM_WINDOW 64
+#define GSSDF_ADAM_MAX_ROW_GROUPS 2
+#define GSSDF_ADAM_ROW_SCALARS 128   /* GSSDF_ADAM_MAX_ROW_GROUPS * GSSDF_ADAM_WINDOW */
+typedef struct gssdf_adam_replay {
+    int32_t *last;                                  /* device [rows] */
+    int32_t step;                                   /* current step: rows are brought up to it (catch-up) or to step - 1 (update) */
+    float beta1, beta2, eps;
+    float step_size[GSSDF_ADAM_ROW_SCALARS];        /* [row group k * WINDOW + s % WINDOW] = (float)(lr_k / (1 - beta1^s)) */
+    float inv_sqrt_bc2[GSSDF_ADAM_WINDOW];          /* [s % WINDOW] = (float)(1 / sqrt(1 - beta2^s)) */
+} gssdf_adam_replay;
+/* Host only: r->step := step and slot step % WINDOW := the scalars of step `step` for the learning rates lr0 / lr1 of row groups 0 / 1,
+   computed exactly as gssdf_adam_step computes them (call once per step, before the step's gssdf_adam_step, below). */
+int gssdf_adam_replay_push(gssdf_adam_replay *r, int32_t step, float lr0, float lr1);
 typedef struct gssdf_view_colors_fwd_args {
     int32_t N, C, K;        /* K = SH bases stored per splat */
     int32_t sh_degree;      /* degree to evaluate, (sh_degree+1)^2 <= K, <= 4 */
@@ -375,7 +393,7 @@ typedef struct gssdf_dssim_loss_args {
     float w_dssim;
     float *loss_out;         /* device float[1], += */
     float *v_out_colors;     /* [C,H,W,4] += (channels 0..2) or NULL (forward only) */
-    void *workspace;         /* >= gssdf_dssim_workspace_bytes (three derivative maps) */
+    void *workspace;         /* >= gssdf_dssim_workspace_bytes (three derivative maps + the loss reduction's 16-byte tail) */
     size_t workspace_bytes;
 } gssdf_dssim_loss_args;
 size_t gssdf_dssim_workspace_bytes(int32_t C, int32_t image_width, int32_t image_height);
@@ -667,7 +685,10 @@ typedef struct gssdf_adam_group {
     int64_t offset, count;   /* slice of the flat buffers */
     float lr;
     int32_t half_shadow;     /* 1: params of this group are mirrored to `table_half` (element i of the group -> table_half[i]) */
+    int32_t row_width;       /* 0: dense group. > 0: ROW group of count / row_width rows, brought current lazily (see gssdf_adam_replay);
+                                every row group of one call has the same number of rows, and they share one step stamp per row */
 } gssdf_adam_group;
+
 typedef struct gssdf_adam_args {
     float *params;           /* flat fp32 parameters */
     float *grads;            /* flat fp32 gradients (same indexing) */
@@ -681,6 +702,15 @@ typedef struct gssdf_adam_args {
     void *table_half;        /* fp16 shadow (half_shadow groups) or NULL */
     const gssdf_sdf_net *net; /* or NULL. Non-NULL (mlp_mode 1): net->mlp must point into `params`; gssdf_sdf_mlp_pack(net, mlp_packed) follows */
     void *mlp_packed;
+    /* row groups (row_width > 0) need `replay` (host pointer, read at the call; replay->step == step). Each row visited is first brought
+       to step - 1 by zero-gradient replays, then takes step t with its gradient, and is stamped t. row_ids given: the rows row_ids[0 ..
+       min(*row_count, row_cap)) are visited and must be distinct, every other row of the row groups must have a zero gradient and
+       keeps its stamp. row_ids NULL: every row is visited (a sweep). */
+    const gssdf_adam_replay *replay;
+    const int64_t *row_ids;
+    const gssdf_counts *row_count; /* device: ->nnz */
+    int32_t row_cap;
+    int32_t replay_only;     /* 1: row groups only, no gradient is read or written: every visited row is brought to `step` by replays */
 } gssdf_adam_args;
 int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream);
 
