@@ -40,6 +40,25 @@ void set_error(const char *fmt, ...);
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Bump carver over a caller's workspace. Each operator lists its regions once, in one layout function: on a null base take() returns
+// null and bytes() is the size to advertise, on the caller's workspace take() returns the same regions' pointers. The running offset
+// is rounded up to `align` after each region.
+class WsLayout {
+  public:
+    explicit WsLayout(void *base) : base_(static_cast<char *>(base)) {}
+    template <typename T>
+    T *take(size_t count, size_t align = 256) {
+        T *p = base_ ? reinterpret_cast<T *>(base_ + off_) : nullptr;
+        off_ = align_up(off_ + count * sizeof(T), align);
+        return p;
+    }
+    size_t bytes() const { return off_; }
+
+  private:
+    char *base_;
+    size_t off_ = 0;
+};
+
 constexpr int kTile = 16;           // GS-SDF renders with tile_size 16 (neural_gaussian.cpp:529)
 constexpr int kRecFloats = 16;      // packed per-splat render record: M[9], opacity, rgb[3], normal[3]
 

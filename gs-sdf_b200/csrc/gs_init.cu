@@ -101,14 +101,26 @@ __global__ void __launch_bounds__(kThreads) rot6d_kernel(int64_t n, const int32_
     for (int k = 0; k < 4; ++k) quat[4 * i + k] = q[k];
 }
 
-size_t ws_bytes(int64_t n) { return 2 * align_up((size_t)n * 7 * sizeof(float), 256); }  // sdf [7n] | y1 [7n]
+struct InitWs {
+    float *s7, *y7;  // sdf and first-layer output of the point and its six offsets
+    size_t bytes;
+};
+
+InitWs init_ws(int64_t n, void *base) {
+    WsLayout L(base);
+    InitWs w;
+    w.s7 = L.take<float>((size_t)n * 7);
+    w.y7 = L.take<float>((size_t)n * 7);
+    w.bytes = L.bytes();
+    return w;
+}
 
 }  // namespace
 }  // namespace gssdf
 
 using namespace gssdf;
 
-extern "C" size_t gssdf_sdf_init_gs_workspace_bytes(int64_t n) { return n < 0 ? 0 : ws_bytes(n); }
+extern "C" size_t gssdf_sdf_init_gs_workspace_bytes(int64_t n) { return n < 0 ? 0 : init_ws(n, nullptr).bytes; }
 
 extern "C" int gssdf_sdf_init_gs(const gssdf_sdf_init_gs_args *a, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a, GSSDF_EINVAL, "sdf_init_gs: null args");
@@ -116,13 +128,12 @@ extern "C" int gssdf_sdf_init_gs(const gssdf_sdf_init_gs_args *a, gssdf_stream_t
     GSSDF_REQUIRE(a->delta > 0.f && std::isfinite(a->delta), GSSDF_EINVAL, "sdf_init_gs: delta must be positive and finite, got %g",
                   (double)a->delta);
     GSSDF_REQUIRE(a->quaternion, GSSDF_EINVAL, "sdf_init_gs: quaternion is required");
-    GSSDF_REQUIRE(a->workspace_bytes >= ws_bytes(a->n) && (a->n == 0 || a->workspace), GSSDF_EINVAL,
-                  "sdf_init_gs: workspace too small (%zu < %zu)", a->workspace_bytes, ws_bytes(a->n));
+    const InitWs w = init_ws(a->n, a->workspace);
+    GSSDF_REQUIRE(a->workspace_bytes >= w.bytes && (a->n == 0 || a->workspace), GSSDF_EINVAL, "sdf_init_gs: workspace too small (%zu < %zu)",
+                  a->workspace_bytes, w.bytes);
     if (a->n == 0) return GSSDF_OK;
     GSSDF_REQUIRE(a->x, GSSDF_EINVAL, "sdf_init_gs: x is required");
     GSSDF_REQUIRE(a->net.table_half && a->net.mlp, GSSDF_EINVAL, "sdf_init_gs: net.table_half and net.mlp are required");
-    float *s7 = (float *)a->workspace;
-    float *y7 = (float *)((char *)a->workspace + ws_bytes(a->n) / 2);
     // get_gradient's six offsets and the bare point in one launch: variant 0 is the point itself, variants 1..6 are +-delta e_k
     gssdf_sdf_fwd_args fa = {};
     fa.net = a->net;
@@ -131,13 +142,13 @@ extern "C" int gssdf_sdf_init_gs(const gssdf_sdf_init_gs_args *a, gssdf_stream_t
     fa.n_variants = 7;
     fa.delta = a->delta;
     fa.n_live = a->n_live;
-    fa.sdf = s7;
-    fa.y1 = y7;
+    fa.sdf = w.s7;
+    fa.y1 = w.y7;
     const int rc = gssdf_sdf_fwd(&fa, stream);
     if (rc) return rc;
     // inv_delta = 1.0 / delta is a C++ double (local_map.cpp:126); each coefficient becomes an fp32 scalar where it meets the tensor
     const double inv_delta = 1.0 / (double)a->delta;
-    init_gs_kernel<<<cdiv(a->n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a->n, a->n_live, s7, y7, (float)(0.5 * inv_delta),
+    init_gs_kernel<<<cdiv(a->n, kThreads), kThreads, 0, (cudaStream_t)stream>>>(a->n, a->n_live, w.s7, w.y7, (float)(0.5 * inv_delta),
                                                                                   (float)(inv_delta * inv_delta), a->bce_isigma, a->grad,
                                                                                   a->curv_dom, a->quaternion, a->opacity);
     GSSDF_LAUNCH_OK("init_gs_kernel");

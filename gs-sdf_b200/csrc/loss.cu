@@ -224,12 +224,24 @@ dssim_bwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, const floa
 
 using namespace gssdf;
 
-// three derivative maps [3][C*3][H][W], then the loss reduction's double sum and warp counter (16-byte aligned tail)
-static size_t dssim_tail_offset(int32_t C, int32_t W, int32_t H) { return ((size_t)9 * C * W * H * sizeof(float) + 15) / 16 * 16; }
+struct DssimWs {
+    float *maps;  // three derivative maps [3][C*3][H][W]
+    char *tail;   // the loss reduction's double sum and warp counter
+    size_t bytes;
+};
+
+static DssimWs dssim_ws(int32_t C, int32_t W, int32_t H, void *base) {
+    WsLayout L(base);
+    DssimWs w;
+    w.maps = L.take<float>((size_t)9 * C * W * H, 16);
+    w.tail = L.take<char>(16, 16);
+    w.bytes = L.bytes();
+    return w;
+}
 
 extern "C" size_t gssdf_dssim_workspace_bytes(int32_t C, int32_t W, int32_t H) {
     if (C <= 0 || W <= 0 || H <= 0) return 0;
-    return dssim_tail_offset(C, W, H) + 16;
+    return dssim_ws(C, W, H, nullptr).bytes;
 }
 
 // rows per band: a warp marches (band + 10) row steps and the launch takes ceil(CTAs / resident CTAs) rounds of them (the kernels
@@ -257,26 +269,24 @@ extern "C" int gssdf_dssim_loss(const gssdf_dssim_loss_args *a, gssdf_stream_t s
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "dssim_loss: null args");
     GSSDF_REQUIRE(a->C > 0 && a->image_width > 0 && a->image_height > 0, GSSDF_EINVAL, "dssim_loss: bad image size");
     GSSDF_REQUIRE(a->out_colors && a->gt && a->loss_out, GSSDF_EINVAL, "dssim_loss: null pointer");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_dssim_workspace_bytes(a->C, a->image_width, a->image_height), GSSDF_ENOMEM,
-                  "dssim_loss: workspace too small");
+    const DssimWs w = dssim_ws(a->C, a->image_width, a->image_height, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "dssim_loss: workspace too small");
     static const SsimWindow win = make_window();
     const double n = (double)a->C * 3.0 * a->image_width * a->image_height;
-    float *maps = reinterpret_cast<float *>(a->workspace);
     cudaStream_t st = (cudaStream_t)stream;
     const int gx = cdiv(cdiv(a->image_width, kStrip), kSsimWarps);
     {
         const int band = ssim_band_height((const void *)dssim_fwd_kernel, a->image_width, a->image_height, a->C);
         const dim3 grid(gx, cdiv(a->image_height, band), a->C * 3);
-        char *tail = reinterpret_cast<char *>(a->workspace) + dssim_tail_offset(a->C, a->image_width, a->image_height);
-        SsimSum red{reinterpret_cast<double *>(tail), reinterpret_cast<unsigned *>(tail + 8),
+        SsimSum red{reinterpret_cast<double *>(w.tail), reinterpret_cast<unsigned *>(w.tail + 8),
                     (unsigned)cdiv(a->image_width, kStrip) * grid.y * grid.z, (double)a->w_dssim / n};
-        GSSDF_CUDA_OK(cudaMemsetAsync(tail, 0, 16, st));
-        dssim_fwd_kernel<<<grid, kSsimWarps * 32, 0, st>>>(*a, win, maps, red, band);
+        GSSDF_CUDA_OK(cudaMemsetAsync(w.tail, 0, 16, st));
+        dssim_fwd_kernel<<<grid, kSsimWarps * 32, 0, st>>>(*a, win, w.maps, red, band);
         GSSDF_LAUNCH_OK("dssim_fwd_kernel");
     }
     if (a->v_out_colors) {
         const int band = ssim_band_height((const void *)dssim_bwd_kernel, a->image_width, a->image_height, a->C);
-        dssim_bwd_kernel<<<dim3(gx, cdiv(a->image_height, band), a->C * 3), kSsimWarps * 32, 0, st>>>(*a, win, maps, (float)(-a->w_dssim / n), band);
+        dssim_bwd_kernel<<<dim3(gx, cdiv(a->image_height, band), a->C * 3), kSsimWarps * 32, 0, st>>>(*a, win, w.maps, (float)(-a->w_dssim / n), band);
         GSSDF_LAUNCH_OK("dssim_bwd_kernel");
     }
     return GSSDF_OK;

@@ -192,24 +192,19 @@ __global__ void __launch_bounds__(kMcThreads) mc_face_kernel(const McGrid g, con
 struct McWorkspace {
     int32_t *blk_v, *blk_t, *vbase;
     uint8_t *vbits;
+    size_t bytes;
 };
 
-size_t mc_ws_layout(int64_t n, void *base, McWorkspace *w) {
+McWorkspace mc_ws(int64_t n, void *base) {
     const int64_t nblk = (n + kMcThreads - 1) / kMcThreads;
-    size_t off = 0;
-    char *b = (char *)base;
-    auto take = [&](size_t bytes) {
-        char *p = b ? b + off : nullptr;
-        off = align_up(off + bytes, 256);
-        return p;
-    };
-    McWorkspace t;
-    t.blk_v = (int32_t *)take(nblk * 4);
-    t.blk_t = (int32_t *)take(nblk * 4);
-    t.vbase = (int32_t *)take(n * 4);
-    t.vbits = (uint8_t *)take(n);
-    if (w) *w = t;
-    return off;
+    WsLayout L(base);
+    McWorkspace w;
+    w.blk_v = L.take<int32_t>(nblk);
+    w.blk_t = L.take<int32_t>(nblk);
+    w.vbase = L.take<int32_t>(n);
+    w.vbits = L.take<uint8_t>(n);
+    w.bytes = L.bytes();
+    return w;
 }
 
 }  // namespace
@@ -219,7 +214,7 @@ using namespace gssdf;
 
 extern "C" size_t gssdf_marching_cubes_workspace_bytes(int32_t nx, int32_t ny, int32_t nz) {
     if (nx <= 0 || ny <= 0 || nz <= 0) return 0;
-    return mc_ws_layout((int64_t)nx * ny * nz, nullptr, nullptr);
+    return mc_ws((int64_t)nx * ny * nz, nullptr).bytes;
 }
 
 extern "C" int gssdf_marching_cubes(const gssdf_marching_cubes_args *a, gssdf_stream_t stream) {
@@ -240,8 +235,8 @@ extern "C" int gssdf_marching_cubes(const gssdf_marching_cubes_args *a, gssdf_st
         return GSSDF_OK;
     }
     GSSDF_REQUIRE(a->grid, GSSDF_EINVAL, "marching_cubes: grid is required");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_marching_cubes_workspace_bytes(a->nx, a->ny, a->nz), GSSDF_ENOMEM,
-                  "marching_cubes: workspace too small");
+    const McWorkspace w = mc_ws(n, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "marching_cubes: workspace too small");
     McGrid g;
     g.nx = a->nx, g.ny = a->ny, g.nz = a->nz, g.n = n, g.v = a->grid, g.thresh = a->thresh;
     const int32_t res[3] = {a->nx, a->ny, a->nz};
@@ -249,8 +244,6 @@ extern "C" int gssdf_marching_cubes(const gssdf_marching_cubes_args *a, gssdf_st
         g.lower[k] = a->lower[k];
         g.scale[k] = (a->upper[k] - a->lower[k]) / (float)res[k];  // the reference computes it on the host in fp32 too
     }
-    McWorkspace w;
-    mc_ws_layout(n, a->workspace, &w);
     const int64_t nblk = (n + kMcThreads - 1) / kMcThreads;
     mc_count_kernel<<<(unsigned)nblk, kMcThreads, 0, s>>>(g, w.blk_v, w.blk_t);
     GSSDF_LAUNCH_OK("mc_count_kernel");

@@ -102,13 +102,23 @@ __global__ void __launch_bounds__(kThreads) face_scatter_kernel(int32_t m, const
     if (j == m - 1) counts[0] = pos[j] + flags[j];
 }
 
-size_t cub_bytes(int64_t m) {
-    size_t b = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, b, (const int32_t *)nullptr, (int32_t *)nullptr, (int)m);
-    return b;
-}
+struct CullWs {
+    int32_t *flags, *pos;
+    void *cub;
+    size_t cub_bytes, bytes;
+};
 
-size_t ws_bytes(int64_t m) { return 2 * align_up((size_t)m * sizeof(int32_t), 256) + align_up(cub_bytes(m), 256); }  // flags | pos | cub
+CullWs cull_ws(int64_t m, void *base) {
+    WsLayout L(base);
+    CullWs w;
+    w.flags = L.take<int32_t>(m);
+    w.pos = L.take<int32_t>(m);
+    w.cub_bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, w.cub_bytes, (const int32_t *)nullptr, (int32_t *)nullptr, (int)m);
+    w.cub = L.take<char>(w.cub_bytes);
+    w.bytes = L.bytes();
+    return w;
+}
 
 }  // namespace
 }  // namespace gssdf
@@ -138,7 +148,7 @@ extern "C" int gssdf_mesh_cull_vertices(const gssdf_mesh_cull_vertices_args *a, 
     return GSSDF_OK;
 }
 
-extern "C" size_t gssdf_mesh_cull_workspace_bytes(int64_t m) { return (m < 0 || m > INT32_MAX) ? 0 : ws_bytes(m); }
+extern "C" size_t gssdf_mesh_cull_workspace_bytes(int64_t m) { return (m < 0 || m > INT32_MAX) ? 0 : cull_ws(m, nullptr).bytes; }
 
 extern "C" int gssdf_mesh_cull_faces(const gssdf_mesh_cull_faces_args *a, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a, GSSDF_EINVAL, "mesh_cull_faces: null args");
@@ -146,22 +156,20 @@ extern "C" int gssdf_mesh_cull_faces(const gssdf_mesh_cull_faces_args *a, gssdf_
     GSSDF_REQUIRE(a->n_vertices >= 0 && a->n_vertices <= INT32_MAX, GSSDF_EINVAL, "mesh_cull_faces: n_vertices must be in [0, 2^31), got %lld",
                   (long long)a->n_vertices);
     GSSDF_REQUIRE(a->counts, GSSDF_EINVAL, "mesh_cull_faces: counts is required");
-    GSSDF_REQUIRE(a->workspace_bytes >= ws_bytes(a->m) && (a->m == 0 || a->workspace), GSSDF_EINVAL,
-                  "mesh_cull_faces: workspace too small (%zu < %zu)", a->workspace_bytes, ws_bytes(a->m));
+    const CullWs w = cull_ws(a->m, a->workspace);
+    GSSDF_REQUIRE(a->workspace_bytes >= w.bytes && (a->m == 0 || a->workspace), GSSDF_EINVAL, "mesh_cull_faces: workspace too small (%zu < %zu)",
+                  a->workspace_bytes, w.bytes);
     GSSDF_REQUIRE(a->m == 0 || (a->faces && a->out && (a->seen || a->n_vertices == 0)), GSSDF_EINVAL,
                   "mesh_cull_faces: faces, out and seen are required");
     const cudaStream_t s = (cudaStream_t)stream;
     GSSDF_CUDA_OK(cudaMemsetAsync(a->counts, 0, 2 * sizeof(int32_t), s));
     if (a->m == 0) return GSSDF_OK;
     const int32_t m = (int32_t)a->m;
-    int32_t *flags = (int32_t *)a->workspace;
-    int32_t *pos = (int32_t *)((char *)a->workspace + align_up((size_t)m * sizeof(int32_t), 256));
-    void *cub_tmp = (char *)a->workspace + 2 * align_up((size_t)m * sizeof(int32_t), 256);
-    size_t cb = cub_bytes(m);
-    face_flags_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, a->faces, (int32_t)a->n_vertices, a->seen, flags, a->counts);
+    size_t cb = w.cub_bytes;
+    face_flags_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, a->faces, (int32_t)a->n_vertices, a->seen, w.flags, a->counts);
     GSSDF_LAUNCH_OK("face_flags_kernel");
-    GSSDF_CUDA_OK(cub::DeviceScan::ExclusiveSum(cub_tmp, cb, flags, pos, m, s));
-    face_scatter_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, a->faces, flags, pos, a->out, a->counts);
+    GSSDF_CUDA_OK(cub::DeviceScan::ExclusiveSum(w.cub, cb, w.flags, w.pos, m, s));
+    face_scatter_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, a->faces, w.flags, w.pos, a->out, a->counts);
     GSSDF_LAUNCH_OK("face_scatter_kernel");
     return GSSDF_OK;
 }

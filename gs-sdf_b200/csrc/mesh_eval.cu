@@ -201,8 +201,22 @@ __global__ void __launch_bounds__(kThreads) scan_apply_kernel(int32_t m, const d
 }
 
 int n_tiles(int64_t m) { return cdiv(m, kScanTile); }
-size_t sample_ws_bytes(int64_t m) {  // area | prefix | ends | tile sums | tile offsets
-    return 3 * align_up((size_t)m * 8, 256) + 2 * align_up((size_t)n_tiles(m) * 8, 256);
+struct SampleWs {
+    double *area, *prefix;
+    int64_t *ends;
+    double *tsum, *toff;  // per scan tile: sums, then their exclusive scan
+    size_t bytes;
+};
+SampleWs sample_ws(int64_t m, void *base) {
+    WsLayout L(base);
+    SampleWs w;
+    w.area = L.take<double>(m);
+    w.prefix = L.take<double>(m);
+    w.ends = L.take<int64_t>(m);
+    w.tsum = L.take<double>(n_tiles(m));
+    w.toff = L.take<double>(n_tiles(m));
+    w.bytes = L.bytes();
+    return w;
 }
 
 // ---------------------------------------------------------------- voxel down-sampling
@@ -318,31 +332,27 @@ struct VoxelWs {
     int32_t *vals_in, *vals_out, *head, *pos, *starts;
     double *partial;
     void *cub;
-    size_t cub_bytes;
+    size_t cub_bytes, bytes;
 };
-size_t voxel_cub_bytes(int64_t cap) {
-    size_t a = 0, b = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, a, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr,
+VoxelWs voxel_ws(int64_t cap, void *base) {
+    WsLayout L(base);
+    VoxelWs w;
+    w.keys_in = L.take<uint64_t>(cap);
+    w.keys_out = L.take<uint64_t>(cap);
+    w.vals_in = L.take<int32_t>(cap);
+    w.vals_out = L.take<int32_t>(cap);
+    w.head = L.take<int32_t>(cap);
+    w.pos = L.take<int32_t>(cap);
+    w.starts = L.take<int32_t>(cap + 1);
+    w.partial = L.take<double>(kMinBlocks * 3);
+    size_t sort_b = 0, scan_b = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const int32_t *)nullptr, (int32_t *)nullptr,
                                     (int)cap);
-    cub::DeviceScan::ExclusiveSum(nullptr, b, (const int32_t *)nullptr, (int32_t *)nullptr, (int)cap);
-    return a > b ? a : b;
-}
-size_t voxel_ws_bytes(int64_t cap, VoxelWs *w = nullptr, void *base = nullptr) {
-    const size_t k8 = align_up((size_t)cap * 8, 256), k4 = align_up((size_t)cap * 4, 256), ks = align_up((size_t)(cap + 1) * 4, 256);
-    const size_t kp = align_up(kMinBlocks * 3 * sizeof(double), 256), cb = voxel_cub_bytes(cap);
-    if (w) {
-        char *p = (char *)base;
-        w->keys_in = (uint64_t *)p, p += k8;
-        w->keys_out = (uint64_t *)p, p += k8;
-        w->vals_in = (int32_t *)p, p += k4;
-        w->vals_out = (int32_t *)p, p += k4;
-        w->head = (int32_t *)p, p += k4;
-        w->pos = (int32_t *)p, p += k4;
-        w->starts = (int32_t *)p, p += ks;
-        w->partial = (double *)p, p += kp;
-        w->cub = p, w->cub_bytes = cb;
-    }
-    return 2 * k8 + 4 * k4 + ks + kp + align_up(cb, 256);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const int32_t *)nullptr, (int32_t *)nullptr, (int)cap);
+    w.cub_bytes = sort_b > scan_b ? sort_b : scan_b;
+    w.cub = L.take<char>(w.cub_bytes);
+    w.bytes = L.bytes();
+    return w;
 }
 
 template <typename T>
@@ -494,14 +504,24 @@ __global__ void __launch_bounds__(kThreads) nn_final_kernel(int32_t n_blocks, co
     }
 }
 
-size_t nn_ws_bytes(int64_t cap_q) { return align_up((size_t)(cap_q > 0 ? cdiv(cap_q, kThreads) : 1) * kPartial * sizeof(double), 256); }
+struct NnWs {
+    double *partial;  // kPartial sums per query block
+    size_t bytes;
+};
+NnWs nn_ws(int64_t cap_q, void *base) {
+    WsLayout L(base);
+    NnWs w;
+    w.partial = L.take<double>((size_t)(cap_q > 0 ? cdiv(cap_q, kThreads) : 1) * kPartial);
+    w.bytes = L.bytes();
+    return w;
+}
 
 }  // namespace
 }  // namespace gssdf
 
 using namespace gssdf;
 
-extern "C" size_t gssdf_mesh_sample_uniform_workspace_bytes(int64_t m) { return (m < 0 || m > INT32_MAX) ? 0 : sample_ws_bytes(m); }
+extern "C" size_t gssdf_mesh_sample_uniform_workspace_bytes(int64_t m) { return (m < 0 || m > INT32_MAX) ? 0 : sample_ws(m, nullptr).bytes; }
 
 extern "C" int gssdf_mesh_sample_uniform(const gssdf_mesh_sample_uniform_args *a, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a, GSSDF_EINVAL, "mesh_sample_uniform: null args");
@@ -511,8 +531,9 @@ extern "C" int gssdf_mesh_sample_uniform(const gssdf_mesh_sample_uniform_args *a
     GSSDF_REQUIRE(a->n_samples >= 0 && a->n_samples <= INT32_MAX, GSSDF_EINVAL,
                   "mesh_sample_uniform: n_samples must be in [0, 2^31), got %lld", (long long)a->n_samples);
     GSSDF_REQUIRE(a->counts, GSSDF_EINVAL, "mesh_sample_uniform: counts is required");
-    GSSDF_REQUIRE(a->workspace_bytes >= sample_ws_bytes(a->m) && (a->m == 0 || a->workspace), GSSDF_EINVAL,
-                  "mesh_sample_uniform: workspace too small (%zu < %zu)", a->workspace_bytes, sample_ws_bytes(a->m));
+    const SampleWs w = sample_ws(a->m, a->workspace);
+    GSSDF_REQUIRE(a->workspace_bytes >= w.bytes && (a->m == 0 || a->workspace), GSSDF_EINVAL,
+                  "mesh_sample_uniform: workspace too small (%zu < %zu)", a->workspace_bytes, w.bytes);
     GSSDF_REQUIRE(a->m == 0 || (a->faces && (a->vertices || a->n_vertices == 0) && (a->samples || a->n_samples == 0)), GSSDF_EINVAL,
                   "mesh_sample_uniform: faces, vertices and samples are required");
     Box box{};
@@ -527,32 +548,28 @@ extern "C" int gssdf_mesh_sample_uniform(const gssdf_mesh_sample_uniform_args *a
     GSSDF_CUDA_OK(cudaMemsetAsync(a->counts, 0, 2 * sizeof(int32_t), s));
     if (a->m == 0) return GSSDF_OK;
     const int32_t m = (int32_t)a->m;
-    const size_t k8 = align_up((size_t)m * 8, 256);
-    double *area = (double *)a->workspace, *prefix = (double *)((char *)a->workspace + k8);
-    int64_t *ends = (int64_t *)((char *)a->workspace + 2 * k8);
     const int nt = n_tiles(m);
-    double *tsum = (double *)((char *)a->workspace + 3 * k8), *toff = tsum + align_up((size_t)nt * 8, 256) / 8;
-    tri_area_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, a->faces, (int32_t)a->n_vertices, a->vertices, a->use_box != 0, box, area,
+    tri_area_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, a->faces, (int32_t)a->n_vertices, a->vertices, a->use_box != 0, box, w.area,
                                                            a->counts);
     GSSDF_LAUNCH_OK("tri_area_kernel");
-    scan_tile_sum_kernel<<<nt, kThreads, 0, s>>>(m, area, tsum);
+    scan_tile_sum_kernel<<<nt, kThreads, 0, s>>>(m, w.area, w.tsum);
     GSSDF_LAUNCH_OK("scan_tile_sum_kernel");
-    scan_tile_offset_kernel<<<1, kThreads, 0, s>>>(nt, tsum, toff);
+    scan_tile_offset_kernel<<<1, kThreads, 0, s>>>(nt, w.tsum, w.toff);
     GSSDF_LAUNCH_OK("scan_tile_offset_kernel");
-    scan_apply_kernel<<<nt, kThreads, 0, s>>>(m, area, toff, prefix);
+    scan_apply_kernel<<<nt, kThreads, 0, s>>>(m, w.area, w.toff, w.prefix);
     GSSDF_LAUNCH_OK("scan_apply_kernel");
-    tri_ends_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, prefix, (double)a->n_samples, ends, a->counts);
+    tri_ends_kernel<<<cdiv(m, kThreads), kThreads, 0, s>>>(m, w.prefix, (double)a->n_samples, w.ends, a->counts);
     GSSDF_LAUNCH_OK("tri_ends_kernel");
     if (a->n_samples == 0) return GSSDF_OK;
     const uint64_t seed = (uint64_t)a->seed;
     const int blocks = cdiv(a->n_samples, kThreads) < 132 * 16 ? cdiv(a->n_samples, kThreads) : 132 * 16;  // grid-stride over the samples
-    sample_kernel<<<blocks, kThreads, 0, s>>>(m, ends, a->faces, a->vertices, (uint32_t)seed,
+    sample_kernel<<<blocks, kThreads, 0, s>>>(m, w.ends, a->faces, a->vertices, (uint32_t)seed,
                                                                                       (uint32_t)(seed >> 32), a->n_samples, a->samples);
     GSSDF_LAUNCH_OK("sample_kernel");
     return GSSDF_OK;
 }
 
-extern "C" size_t gssdf_voxel_downsample_workspace_bytes(int64_t cap) { return (cap < 0 || cap > INT32_MAX - 1) ? 0 : voxel_ws_bytes(cap); }
+extern "C" size_t gssdf_voxel_downsample_workspace_bytes(int64_t cap) { return (cap < 0 || cap > INT32_MAX - 1) ? 0 : voxel_ws(cap, nullptr).bytes; }
 
 extern "C" int gssdf_voxel_downsample(const gssdf_voxel_downsample_args *a, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a, GSSDF_EINVAL, "voxel_downsample: null args");
@@ -562,20 +579,19 @@ extern "C" int gssdf_voxel_downsample(const gssdf_voxel_downsample_args *a, gssd
                   (int)a->dtype);
     GSSDF_REQUIRE(a->voxel_size > 0.0 && isfinite(a->voxel_size), GSSDF_EINVAL, "voxel_downsample: voxel_size must be positive and finite");
     GSSDF_REQUIRE(a->counts && a->origin, GSSDF_EINVAL, "voxel_downsample: counts and origin are required");
-    GSSDF_REQUIRE(a->workspace_bytes >= voxel_ws_bytes(a->cap) && a->workspace, GSSDF_EINVAL, "voxel_downsample: workspace too small (%zu < %zu)",
-                  a->workspace_bytes, voxel_ws_bytes(a->cap));
+    const VoxelWs w = voxel_ws(a->cap, a->workspace);
+    GSSDF_REQUIRE(a->workspace_bytes >= w.bytes && a->workspace, GSSDF_EINVAL, "voxel_downsample: workspace too small (%zu < %zu)",
+                  a->workspace_bytes, w.bytes);
     GSSDF_REQUIRE(a->cap == 0 || (a->points && a->out_points && a->out_keys), GSSDF_EINVAL,
                   "voxel_downsample: points, out_points and out_keys are required");
     const cudaStream_t s = (cudaStream_t)stream;
     GSSDF_CUDA_OK(cudaMemsetAsync(a->counts, 0, 2 * sizeof(int32_t), s));
     if (a->cap == 0) return GSSDF_OK;
-    VoxelWs w;
-    voxel_ws_bytes(a->cap, &w, a->workspace);
     return a->dtype == 0 ? voxel_downsample<float>(a, w, s) : voxel_downsample<double>(a, w, s);
 }
 
 extern "C" size_t gssdf_nn_truncated_workspace_bytes(int64_t cap_queries) {
-    return (cap_queries < 0 || cap_queries > INT32_MAX) ? 0 : nn_ws_bytes(cap_queries);
+    return (cap_queries < 0 || cap_queries > INT32_MAX) ? 0 : nn_ws(cap_queries, nullptr).bytes;
 }
 
 extern "C" int gssdf_nn_truncated(const gssdf_nn_truncated_args *a, gssdf_stream_t stream) {
@@ -592,8 +608,9 @@ extern "C" int gssdf_nn_truncated(const gssdf_nn_truncated_args *a, gssdf_stream
     GSSDF_REQUIRE(a->trunc / H <= 1024.0, GSSDF_EINVAL, "nn_truncated: trunc / (voxel_size * 2^cell_shift) = %g exceeds 1024 rings",
                   a->trunc / H);
     GSSDF_REQUIRE(a->result, GSSDF_EINVAL, "nn_truncated: result is required");
-    GSSDF_REQUIRE(a->workspace_bytes >= nn_ws_bytes(a->cap_queries) && a->workspace, GSSDF_EINVAL, "nn_truncated: workspace too small (%zu < %zu)",
-                  a->workspace_bytes, nn_ws_bytes(a->cap_queries));
+    const NnWs w = nn_ws(a->cap_queries, a->workspace);
+    GSSDF_REQUIRE(a->workspace_bytes >= w.bytes && a->workspace, GSSDF_EINVAL, "nn_truncated: workspace too small (%zu < %zu)", a->workspace_bytes,
+                  w.bytes);
     GSSDF_REQUIRE((a->cap_queries == 0 || (a->queries && a->target_origin)) && (a->cap_targets == 0 || (a->targets && a->target_keys)),
                   GSSDF_EINVAL, "nn_truncated: queries, targets, target_keys and target_origin are required");
     const cudaStream_t s = (cudaStream_t)stream;
@@ -604,11 +621,10 @@ extern "C" int gssdf_nn_truncated(const gssdf_nn_truncated_args *a, gssdf_stream
     g.trunc = a->trunc, g.trunc2 = a->trunc * a->trunc, g.thresh = a->threshold, g.slack = H * 1e-9;
     g.rings = (int)ceil(a->trunc / H) + 1, g.clamp = a->clamp_beyond != 0;
     const int nb = cdiv(a->cap_queries, kThreads);
-    double *partial = (double *)a->workspace;
     nn_kernel<<<nb, kThreads, 0, s>>>(a->cap_queries, a->queries, a->n_queries, a->cap_targets, a->targets, a->target_keys, a->n_targets,
-                                      a->target_origin, g, a->distances, partial);
+                                      a->target_origin, g, a->distances, w.partial);
     GSSDF_LAUNCH_OK("nn_kernel");
-    nn_final_kernel<<<1, kThreads, 0, s>>>(nb, partial, a->result);
+    nn_final_kernel<<<1, kThreads, 0, s>>>(nb, w.partial, a->result);
     GSSDF_LAUNCH_OK("nn_final_kernel");
     return GSSDF_OK;
 }

@@ -586,7 +586,7 @@ static int run_scan(const int32_t *in, int32_t *out, int64_t n, const int32_t *n
     GSSDF_LAUNCH_OK("scan_chunk_apply_kernel");
     return GSSDF_OK;
 }
-static size_t scan_scratch_bytes(int64_t n) { return align_up((size_t)(2 * (n / kScanChunk + 2)) * 4, 256); }
+static size_t scan_scratch_ints(int64_t n) { return (size_t)(2 * (n / kScanChunk + 2)); }  // run_scan's chunk sums and their scan
 
 static int check_tree(const char *who, const gssdf_octree &t) {
     GSSDF_REQUIRE(t.level >= 0 && t.level <= kMaxOctLevel, GSSDF_EINVAL, "%s: octree level out of range", who);
@@ -611,27 +611,40 @@ extern "C" int gssdf_octree_query(const gssdf_octree_query_args *a, gssdf_stream
     return GSSDF_OK;
 }
 
-static size_t ray_ws_bytes(int64_t n_rays) {  // [cnt | off] + the staging slots
+struct RayWs {
+    int32_t *cnt, *off;  // hits per ray and their exclusive scan, back to back
+    StagedHit *stage;    // the first kStageHits hits of every ray
+};
+
+// the ray-trace regions, taken by both ray-trace operators
+static RayWs take_ray_ws(WsLayout &L, int64_t n_rays) {
     const size_t n = (size_t)std::max<int64_t>(n_rays, 1);
-    return align_up(n * 8, 256) + align_up(n * kStageHits * sizeof(StagedHit), 256);
+    RayWs w;
+    w.cnt = L.take<int32_t>(n, alignof(int32_t));
+    w.off = L.take<int32_t>(n);
+    w.stage = L.take<StagedHit>(n * kStageHits);
+    return w;
 }
-extern "C" size_t gssdf_octree_raytrace_workspace_bytes(int64_t n_rays) { return ray_ws_bytes(n_rays); }
+extern "C" size_t gssdf_octree_raytrace_workspace_bytes(int64_t n_rays) {
+    WsLayout L(nullptr);
+    take_ray_ws(L, n_rays);
+    return L.bytes();
+}
 
 static int raytrace_impl(const gssdf_octree &tree, int64_t n_rays, const float *origins, const float *dirs, int64_t cap, int32_t *ridx, int32_t *pidx,
-                         float *depth, int32_t *n_nuggets, int32_t *overflow, int32_t *ws, cudaStream_t st) {
-    int32_t *cnt = ws, *off = ws + n_rays;
-    StagedHit *stage = reinterpret_cast<StagedHit *>(reinterpret_cast<unsigned char *>(ws) + align_up((size_t)std::max<int64_t>(n_rays, 1) * 8, 256));
+                         float *depth, int32_t *n_nuggets, int32_t *overflow, const RayWs &w, cudaStream_t st) {
     GSSDF_CUDA_OK(cudaMemsetAsync(n_nuggets, 0, sizeof(int32_t), st));
     if (n_rays == 0 || tree.n_nodes == 0) return GSSDF_OK;
     const int n_cached = std::min(tree.n_nodes, kTreeCacheNodes);
     const size_t smem = (size_t)n_cached * 5 + 16;
     GSSDF_CUDA_OK(cudaFuncSetAttribute(ray_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTreeCacheNodes * 5 + 16));
     GSSDF_CUDA_OK(cudaFuncSetAttribute(ray_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTreeCacheNodes * 5 + 16));
-    ray_count_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, origins, dirs, cnt, stage);
+    ray_count_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, origins, dirs, w.cnt, w.stage);
     GSSDF_LAUNCH_OK("ray_count_kernel");
-    scan_kernel<<<1, 1024, 0, st>>>(cnt, off, n_rays, nullptr, cap, n_nuggets, overflow);
+    scan_kernel<<<1, 1024, 0, st>>>(w.cnt, w.off, n_rays, nullptr, cap, n_nuggets, overflow);
     GSSDF_LAUNCH_OK("scan_kernel");
-    ray_write_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, origins, dirs, cnt, off, stage, cap, ridx, pidx, depth);
+    ray_write_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, origins, dirs, w.cnt, w.off, w.stage, cap, ridx,
+                                                                          pidx, depth);
     GSSDF_LAUNCH_OK("ray_write_kernel");
     return GSSDF_OK;
 }
@@ -643,21 +656,41 @@ extern "C" int gssdf_octree_raytrace(const gssdf_octree_raytrace_args *a, gssdf_
     if (rc) return rc;
     GSSDF_REQUIRE(a->n_nuggets != nullptr, GSSDF_EINVAL, "octree_raytrace: n_nuggets null");
     GSSDF_REQUIRE(a->n_rays == 0 || (a->origins && a->dirs && a->ridx && a->depth), GSSDF_EINVAL, "octree_raytrace: null pointer");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_octree_raytrace_workspace_bytes(a->n_rays), GSSDF_ENOMEM, "octree_raytrace: workspace too small");
+    WsLayout L(a->workspace);
+    const RayWs w = take_ray_ws(L, a->n_rays);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= L.bytes(), GSSDF_ENOMEM, "octree_raytrace: workspace too small");
     GSSDF_CUDA_OK(cudaMemsetAsync(a->n_nuggets, 0, 2 * sizeof(int32_t), (cudaStream_t)stream));
-    return raytrace_impl(a->tree, a->n_rays, a->origins, a->dirs, a->cap, a->ridx, a->pidx, a->depth, a->n_nuggets, a->n_nuggets + 1,
-                         reinterpret_cast<int32_t *>(a->workspace), (cudaStream_t)stream);
+    return raytrace_impl(a->tree, a->n_rays, a->origins, a->dirs, a->cap, a->ridx, a->pidx, a->depth, a->n_nuggets, a->n_nuggets + 1, w,
+                         (cudaStream_t)stream);
 }
 
 static int64_t sample_cand_cap(int64_t n_rays, int64_t nugget_cap, int ns, int n_free, int n_surface) {
     return nugget_cap * ns + n_rays * ((int64_t)n_free + n_surface + 1);
 }
 
+struct SampleRaysWs {
+    RayWs ray;
+    int32_t *nug_ridx;
+    float *nug_depth;  // entry and exit depth per nugget
+    int32_t *flags, *pos, *scan_scratch;  // per candidate
+    size_t bytes;
+};
+
+static SampleRaysWs sample_rays_ws(int64_t n_rays, int64_t nugget_cap, int64_t m, void *base) {
+    WsLayout L(base);
+    SampleRaysWs w;
+    w.ray = take_ray_ws(L, n_rays);
+    w.nug_ridx = L.take<int32_t>(nugget_cap);
+    w.nug_depth = L.take<float>(nugget_cap * 2);
+    w.flags = L.take<int32_t>(m);
+    w.pos = L.take<int32_t>(m);
+    w.scan_scratch = L.take<int32_t>(scan_scratch_ints(m));
+    w.bytes = L.bytes();
+    return w;
+}
+
 extern "C" size_t gssdf_sdf_sample_rays_workspace_bytes(int64_t n_rays, int64_t nugget_cap, int32_t ns, int32_t n_free, int32_t n_surface) {
-    const int64_t m = sample_cand_cap(n_rays, nugget_cap, ns, n_free, n_surface);
-    // ray traversal scratch, nuggets (ridx, depth x2), flags + positions per candidate, scan scratch
-    return ray_ws_bytes(n_rays) + align_up((size_t)nugget_cap * 4, 256) + align_up((size_t)nugget_cap * 8, 256) + 2 * align_up((size_t)m * 4, 256) +
-           scan_scratch_bytes(m);
+    return sample_rays_ws(n_rays, nugget_cap, sample_cand_cap(n_rays, nugget_cap, ns, n_free, n_surface), nullptr).bytes;
 }
 
 extern "C" int gssdf_sdf_sample_rays(const gssdf_sdf_sample_rays_args *a, gssdf_stream_t stream) {
@@ -673,36 +706,42 @@ extern "C" int gssdf_sdf_sample_rays(const gssdf_sdf_sample_rays_args *a, gssdf_
     GSSDF_REQUIRE(a->origin && a->direction && a->depth && a->xyz && a->out_xyz && a->out_ray_sdf, GSSDF_EINVAL, "sdf_sample_rays: null pointer");
     GSSDF_REQUIRE(a->rand_voxel && (a->n_free == 0 || a->rand_free) && (a->n_surface == 0 || a->randn_surface), GSSDF_EINVAL,
                   "sdf_sample_rays: the random draws are inputs (rand_voxel / rand_free / randn_surface)");
-    const size_t need = gssdf_sdf_sample_rays_workspace_bytes(a->n_rays, a->nugget_cap, a->voxel_sample_num, a->n_free, a->n_surface);
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= need, GSSDF_ENOMEM, "sdf_sample_rays: workspace too small (%zu < %zu)", a->workspace_bytes, need);
     const int64_t m_cap = sample_cand_cap(a->n_rays, a->nugget_cap, a->voxel_sample_num, a->n_free, a->n_surface);
+    const SampleRaysWs w = sample_rays_ws(a->n_rays, a->nugget_cap, m_cap, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "sdf_sample_rays: workspace too small (%zu < %zu)", a->workspace_bytes,
+                  w.bytes);
     GSSDF_REQUIRE(m_cap < ((int64_t)1 << 31), GSSDF_EINVAL, "sdf_sample_rays: too many candidates for one call");
-    unsigned char *w = reinterpret_cast<unsigned char *>(a->workspace);
-    int32_t *ray_ws = reinterpret_cast<int32_t *>(w);
-    w += ray_ws_bytes(a->n_rays);
-    int32_t *nug_ridx = reinterpret_cast<int32_t *>(w);
-    w += align_up((size_t)a->nugget_cap * 4, 256);
-    float *nug_depth = reinterpret_cast<float *>(w);
-    w += align_up((size_t)a->nugget_cap * 8, 256);
-    int32_t *flags = reinterpret_cast<int32_t *>(w);
-    w += align_up((size_t)m_cap * 4, 256);
-    int32_t *pos = reinterpret_cast<int32_t *>(w);
-    w += align_up((size_t)m_cap * 4, 256);
-    int32_t *scan_scratch = reinterpret_cast<int32_t *>(w);
-    rc = raytrace_impl(a->tree, a->n_rays, a->origin, a->direction, a->nugget_cap, nug_ridx, nullptr, nug_depth, a->counts + 1, a->counts + 2, ray_ws, st);
+    rc = raytrace_impl(a->tree, a->n_rays, a->origin, a->direction, a->nugget_cap, w.nug_ridx, nullptr, w.nug_depth, a->counts + 1, a->counts + 2,
+                       w.ray, st);
     if (rc) return rc;
-    sample_flag_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, nug_ridx, nug_depth, flags, m_cap);
+    sample_flag_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, w.nug_ridx, w.nug_depth, w.flags, m_cap);
     GSSDF_LAUNCH_OK("sample_flag_kernel");
-    rc = run_scan(flags, pos, m_cap, nullptr, a->cap, a->counts, a->counts + 2, scan_scratch, st);
+    rc = run_scan(w.flags, w.pos, m_cap, nullptr, a->cap, a->counts, a->counts + 2, w.scan_scratch, st);
     if (rc) return rc;
-    sample_write_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, nug_ridx, nug_depth, flags, pos, m_cap);
+    sample_write_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, w.nug_ridx, w.nug_depth, w.flags, w.pos, m_cap);
     GSSDF_LAUNCH_OK("sample_write_kernel");
     return GSSDF_OK;
 }
 
-extern "C" size_t gssdf_sdf_gate_compact_workspace_bytes(int64_t n) {
-    return 2 * align_up((size_t)std::max<int64_t>(n, 1) * 4, 256) + scan_scratch_bytes(n) + 256;
+struct GateWs {
+    int32_t *flags, *pos;
+    int32_t *scratch_ovf;  // never set: the count cannot exceed n
+    int32_t *scan_scratch;
+    size_t bytes;
+};
+
+static GateWs gate_ws(int64_t n, void *base) {
+    WsLayout L(base);
+    GateWs w;
+    w.flags = L.take<int32_t>(std::max<int64_t>(n, 1));
+    w.pos = L.take<int32_t>(std::max<int64_t>(n, 1));
+    w.scratch_ovf = L.take<int32_t>(1);
+    w.scan_scratch = L.take<int32_t>(scan_scratch_ints(n));
+    w.bytes = L.bytes();
+    return w;
 }
+
+extern "C" size_t gssdf_sdf_gate_compact_workspace_bytes(int64_t n) { return gate_ws(n, nullptr).bytes; }
 
 extern "C" int gssdf_sdf_gate_compact(const gssdf_sdf_gate_compact_args *a, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a != nullptr && a->n_gate != nullptr, GSSDF_EINVAL, "sdf_gate_compact: null args / n_gate");
@@ -711,19 +750,15 @@ extern "C" int gssdf_sdf_gate_compact(const gssdf_sdf_gate_compact_args *a, gssd
     GSSDF_CUDA_OK(cudaMemsetAsync(a->n_gate, 0, sizeof(int32_t), st));
     if (a->n == 0) return GSSDF_OK;
     GSSDF_REQUIRE(a->x && a->index && a->x_out, GSSDF_EINVAL, "sdf_gate_compact: null pointer");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_sdf_gate_compact_workspace_bytes(a->n), GSSDF_ENOMEM, "sdf_gate_compact: workspace too small");
-    int32_t *flags = reinterpret_cast<int32_t *>(a->workspace);
-    int32_t *pos = reinterpret_cast<int32_t *>(reinterpret_cast<unsigned char *>(a->workspace) + align_up((size_t)a->n * 4, 256));
-    unsigned char *tail = reinterpret_cast<unsigned char *>(a->workspace) + 2 * align_up((size_t)a->n * 4, 256);
-    int32_t *scratch_ovf = reinterpret_cast<int32_t *>(tail);  // never set: the count cannot exceed n
-    int32_t *scan_scratch = reinterpret_cast<int32_t *>(tail + 256);
-    gate_flag_kernel<<<cdiv(a->n, 256), 256, 0, st>>>(*a, flags);
+    const GateWs w = gate_ws(a->n, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "sdf_gate_compact: workspace too small");
+    gate_flag_kernel<<<cdiv(a->n, 256), 256, 0, st>>>(*a, w.flags);
     GSSDF_LAUNCH_OK("gate_flag_kernel");
     {
-        const int rc2 = run_scan(flags, pos, a->n, a->n_live, a->n + 1, a->n_gate, scratch_ovf, scan_scratch, st);
+        const int rc2 = run_scan(w.flags, w.pos, a->n, a->n_live, a->n + 1, a->n_gate, w.scratch_ovf, w.scan_scratch, st);
         if (rc2) return rc2;
     }
-    gate_gather_kernel<<<cdiv(a->n, 256), 256, 0, st>>>(*a, flags, pos);
+    gate_gather_kernel<<<cdiv(a->n, 256), 256, 0, st>>>(*a, w.flags, w.pos);
     GSSDF_LAUNCH_OK("gate_gather_kernel");
     return GSSDF_OK;
 }

@@ -32,10 +32,13 @@ struct Levels {
 
 struct Layout {
     Levels lv;
-    size_t bm_bytes, raw_off, cnt_off, pre_off, cub_off, cub_bytes, total;
+    uint64_t *bm, *raw;  // bitmaps of every level, then the raw leaf bitmap: call 1 clears [0, cleared_bytes)
+    int64_t *cnt, *pre;
+    void *cub;
+    size_t cleared_bytes, cub_bytes, bytes;
 };
 
-Layout layout(int level) {
+Layout layout(int level, void *base) {
     Layout o;
     o.lv.L = level;
     int64_t s = 0;
@@ -45,14 +48,16 @@ Layout layout(int level) {
     }
     o.lv.s[level + 1] = s;
     const int64_t leaf_sb = s - o.lv.s[level];
-    o.bm_bytes = (size_t)s * kSbWords * 8;
-    o.raw_off = o.bm_bytes;
-    o.cnt_off = o.raw_off + (size_t)leaf_sb * kSbWords * 8;
-    o.pre_off = o.cnt_off + align_up((size_t)(s + 1) * 8, 256);
-    o.cub_off = o.pre_off + align_up((size_t)(s + 1) * 8, 256);
+    WsLayout L(base);
+    o.bm = L.take<uint64_t>((size_t)s * kSbWords, alignof(uint64_t));
+    o.raw = L.take<uint64_t>((size_t)leaf_sb * kSbWords, alignof(uint64_t));
+    o.cleared_bytes = L.bytes();
+    o.cnt = L.take<int64_t>(s + 1);
+    o.pre = L.take<int64_t>(s + 1);
     o.cub_bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, o.cub_bytes, (const int64_t *)nullptr, (int64_t *)nullptr, (int)(s + 1));
-    o.total = o.cub_off + align_up(o.cub_bytes, 256);
+    o.cub = L.take<char>(o.cub_bytes);
+    o.bytes = L.bytes();
     return o;
 }
 
@@ -267,7 +272,7 @@ int grid_for(int64_t threads, int cap) { return (int)std::max<int64_t>(1, std::m
 using namespace gssdf;
 
 extern "C" size_t gssdf_octree_build_workspace_bytes(int64_t n, int32_t level) {
-    return (n < 0 || level < 1 || level > kMaxBuildLevel) ? 0 : layout(level).total;
+    return (n < 0 || level < 1 || level > kMaxBuildLevel) ? 0 : layout(level, nullptr).bytes;
 }
 
 extern "C" int gssdf_octree_build(const gssdf_octree_build_device_args *a, gssdf_stream_t stream) {
@@ -279,17 +284,16 @@ extern "C" int gssdf_octree_build(const gssdf_octree_build_device_args *a, gssdf
     GSSDF_REQUIRE(a->n == 0 || a->xyz, GSSDF_EINVAL, "octree_build: xyz is required");
     GSSDF_REQUIRE(a->counts, GSSDF_EINVAL, "octree_build: counts is required");
     GSSDF_REQUIRE(a->workspace, GSSDF_EINVAL, "octree_build: workspace is required");
-    const Layout o = layout(a->level);
-    GSSDF_REQUIRE(a->workspace_bytes >= o.total, GSSDF_ENOMEM, "octree_build: workspace too small (%zu < %zu)", a->workspace_bytes, o.total);
+    const Layout o = layout(a->level, a->workspace);
+    GSSDF_REQUIRE(a->workspace_bytes >= o.bytes, GSSDF_ENOMEM, "octree_build: workspace too small (%zu < %zu)", a->workspace_bytes, o.bytes);
     const bool compact = a->octree != nullptr;
     if (compact) {
         GSSDF_REQUIRE(a->node_cap >= 0 && a->point_cap >= 0, GSSDF_EINVAL, "octree_build: capacities must be >= 0");
         GSSDF_REQUIRE(a->exsum && a->points && a->pyramid, GSSDF_EINVAL, "octree_build: exsum, points and pyramid are required with octree");
     }
     const cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)a->workspace;
-    uint64_t *bm = (uint64_t *)ws;
-    int64_t *cnt = (int64_t *)(ws + o.cnt_off), *pre = (int64_t *)(ws + o.pre_off);
+    uint64_t *bm = o.bm;
+    int64_t *cnt = o.cnt, *pre = o.pre;
     const Levels &lv = o.lv;
     const int L = a->level;
     if (compact) {
@@ -301,8 +305,8 @@ extern "C" int gssdf_octree_build(const gssdf_octree_build_device_args *a, gssdf
         return GSSDF_OK;
     }
     // call 1: bitmaps of every level plus the raw one are cleared; the raw one only takes points when they are dilated afterwards
-    GSSDF_CUDA_OK(cudaMemsetAsync(ws, 0, o.cnt_off, st));
-    uint64_t *leaf = bm + lv.s[L] * kSbWords, *raw = (uint64_t *)(ws + o.raw_off);
+    GSSDF_CUDA_OK(cudaMemsetAsync(bm, 0, o.cleared_bytes, st));
+    uint64_t *leaf = bm + lv.s[L] * kSbWords, *raw = o.raw;
     const int64_t leaf_words = (lv.s[L + 1] - lv.s[L]) * kSbWords;
     MarkParams p;
     for (int k = 0; k < 3; ++k) p.org[k] = a->origin[k], p.lo[k] = a->lo[k], p.hi[k] = a->hi[k];
@@ -325,7 +329,7 @@ extern "C" int gssdf_octree_build(const gssdf_octree_build_device_args *a, gssdf
     root_kernel<<<1, 32, 0, st>>>(bm, cnt, lv.s[L + 1]);
     GSSDF_LAUNCH_OK("root_kernel");
     size_t cb = o.cub_bytes;
-    GSSDF_CUDA_OK(cub::DeviceScan::ExclusiveSum((void *)(ws + o.cub_off), cb, cnt, pre, (int)(lv.s[L + 1] + 1), st));
+    GSSDF_CUDA_OK(cub::DeviceScan::ExclusiveSum(o.cub, cb, cnt, pre, (int)(lv.s[L + 1] + 1), st));
     counts_kernel<<<1, 32, 0, st>>>(lv, pre, a->counts);
     GSSDF_LAUNCH_OK("counts_kernel");
     return GSSDF_OK;

@@ -406,10 +406,22 @@ project2dgs_bwd_kernel(const gssdf_project2dgs_bwd_args a) {
 
 using namespace gssdf;
 
-extern "C" size_t gssdf_project2dgs_workspace_bytes(int32_t N, int32_t C) {
+struct ProjectWs {
+    int32_t *cnts, *offs;  // per-block counts, then their exclusive scan (nb + 2) right behind them
+    size_t bytes;
+};
+
+static ProjectWs project_ws(int32_t N, int32_t C, void *base) {
     const size_t nb = (size_t)cdiv(N > 0 ? N : 1, kProjThreads) * (size_t)(C > 0 ? C : 1);
-    return align_up((2 * nb + 2) * sizeof(int32_t), 256);
+    WsLayout L(base);
+    ProjectWs w;
+    w.cnts = L.take<int32_t>(nb, alignof(int32_t));
+    w.offs = L.take<int32_t>(nb + 2);
+    w.bytes = L.bytes();
+    return w;
 }
+
+extern "C" size_t gssdf_project2dgs_workspace_bytes(int32_t N, int32_t C) { return project_ws(N, C, nullptr).bytes; }
 
 static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
@@ -431,19 +443,17 @@ extern "C" int gssdf_project2dgs_fwd(const gssdf_project2dgs_fwd_args *a, gssdf_
                       a->normals,
                   GSSDF_EINVAL, "project2dgs_fwd: packed outputs must be non-null");
     GSSDF_REQUIRE(!a->pt_opacities || a->opacities, GSSDF_EINVAL, "project2dgs_fwd: pt_opacities requires opacities");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_project2dgs_workspace_bytes(a->N, a->C), GSSDF_ENOMEM,
-                  "project2dgs_fwd: workspace too small (%zu < %zu)", a->workspace_bytes,
-                  gssdf_project2dgs_workspace_bytes(a->N, a->C));
+    const ProjectWs w = project_ws(a->N, a->C, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "project2dgs_fwd: workspace too small (%zu < %zu)",
+                  a->workspace_bytes, w.bytes);
     const int bpr = cdiv(a->N, kProjThreads);
     const int nb = bpr * a->C;
-    int32_t *cnts = reinterpret_cast<int32_t *>(a->workspace);
-    int32_t *offs = cnts + nb;
     dim3 grid(bpr, a->C);
-    project2dgs_fwd_kernel<false><<<grid, kProjThreads, 0, st>>>(*a, cnts, nullptr);
+    project2dgs_fwd_kernel<false><<<grid, kProjThreads, 0, st>>>(*a, w.cnts, nullptr);
     GSSDF_LAUNCH_OK("project2dgs_fwd_kernel<count>");
-    scan_block_counts_kernel<<<1, 1024, 0, st>>>(cnts, offs, nb, a->counts, a->cap);
+    scan_block_counts_kernel<<<1, 1024, 0, st>>>(w.cnts, w.offs, nb, a->counts, a->cap);
     GSSDF_LAUNCH_OK("scan_block_counts_kernel");
-    project2dgs_fwd_kernel<true><<<grid, kProjThreads, 0, st>>>(*a, nullptr, offs);
+    project2dgs_fwd_kernel<true><<<grid, kProjThreads, 0, st>>>(*a, nullptr, w.offs);
     GSSDF_LAUNCH_OK("project2dgs_fwd_kernel<write>");
     return GSSDF_OK;
 }

@@ -671,6 +671,7 @@ extern "C" int gssdf_l1_loss(const gssdf_l1_loss_args *a, gssdf_stream_t stream)
     return GSSDF_OK;
 }
 
+// the forward's regions are a prefix of the backward's: reuse_fwd reads the forward's records from the backward's workspace
 struct RasterWs {
     float4 *rec;
     float4 *conic;
@@ -680,27 +681,26 @@ struct RasterWs {
     size_t fwd_bytes, bwd_bytes;
 };
 
-static RasterWs carve_ws(void *base, int C, int W, int H, int cap, int64_t isect_cap) {
+static RasterWs raster_ws(int C, int W, int H, int cap, int64_t isect_cap, void *base) {
     const size_t n = (size_t)(cap > 0 ? cap : 1), I = (size_t)(isect_cap > 0 ? isect_cap : 1);
     const size_t tiles = (size_t)(C > 0 ? C : 1) * cdiv(W > 0 ? W : 1, kTile) * cdiv(H > 0 ? H : 1, kTile);
-    char *p = reinterpret_cast<char *>(base);
+    WsLayout L(base);
     RasterWs w;
-    size_t off = 0;
-    w.rec = reinterpret_cast<float4 *>(p + off); off += align_up(n * kRecBytes, 256);
-    w.conic = reinterpret_cast<float4 *>(p + off); off += align_up(n * kConicF4 * 16, 256);
-    w.clist = reinterpret_cast<int2 *>(p + off); off += align_up(I * sizeof(int2), 256);
-    w.ccount = reinterpret_cast<int32_t *>(p + off); off += align_up(tiles * sizeof(int32_t), 256);
-    w.fwd_bytes = off;
-    w.vrec = reinterpret_cast<float4 *>(p + off); off += align_up(n * 64, 256);
-    w.bwd_bytes = off;
+    w.rec = L.take<float4>(n * kRecF4);
+    w.conic = L.take<float4>(n * kConicF4);
+    w.clist = L.take<int2>(I);
+    w.ccount = L.take<int32_t>(tiles);
+    w.fwd_bytes = L.bytes();
+    w.vrec = L.take<float4>(n * 4);  // 16 gradient floats per splat
+    w.bwd_bytes = L.bytes();
     return w;
 }
 
 extern "C" size_t gssdf_raster2dgs_workspace_bytes(int32_t C, int32_t W, int32_t H, int32_t cap, int64_t isect_cap) {
-    return carve_ws(nullptr, C, W, H, cap, isect_cap).fwd_bytes;
+    return raster_ws(C, W, H, cap, isect_cap, nullptr).fwd_bytes;
 }
 extern "C" size_t gssdf_raster2dgs_bwd_workspace_bytes(int32_t C, int32_t W, int32_t H, int32_t cap, int64_t isect_cap) {
-    return carve_ws(nullptr, C, W, H, cap, isect_cap).bwd_bytes;
+    return raster_ws(C, W, H, cap, isect_cap, nullptr).bwd_bytes;
 }
 
 static int check_raster_common(const char *who, int C, int W, int H, int tile_size, int channels) {
@@ -750,12 +750,10 @@ extern "C" int gssdf_raster2dgs_fwd(const gssdf_raster2dgs_fwd_args *a, gssdf_st
     GSSDF_REQUIRE(a->cap == 0 || (a->ray_transforms && a->colors && a->opacities && a->normals && a->flatten_ids && a->visibilities),
                   GSSDF_EINVAL, "raster2dgs_fwd: null splat input");
     GSSDF_REQUIRE(a->isect_cap >= 0, GSSDF_EINVAL, "raster2dgs_fwd: negative isect_cap");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_raster2dgs_workspace_bytes(a->C, a->image_width, a->image_height, a->cap,
-                                                                                         a->isect_cap),
-                  GSSDF_ENOMEM, "raster2dgs_fwd: workspace too small");
+    const RasterWs w = raster_ws(a->C, a->image_width, a->image_height, a->cap, a->isect_cap, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.fwd_bytes, GSSDF_ENOMEM, "raster2dgs_fwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const int tw = cdiv(a->image_width, kTile), th = cdiv(a->image_height, kTile);
-    const RasterWs w = carve_ws(a->workspace, a->C, a->image_width, a->image_height, a->cap, a->isect_cap);
     rc = pack_and_cull("raster2dgs_fwd", w, a->counts, a->C, a->image_width, a->image_height, a->cap, a->ray_transforms, a->colors,
                        a->opacities, a->normals, a->offsets, a->flatten_ids, a->visibilities, 1, st);
     if (rc) return rc;
@@ -784,12 +782,10 @@ extern "C" int gssdf_raster2dgs_bwd(const gssdf_raster2dgs_bwd_args *a, gssdf_st
                   GSSDF_EINVAL, "raster2dgs_bwd: null input");
     GSSDF_REQUIRE(a->v_ray_transforms && a->v_colors && a->v_opacities && a->v_normals, GSSDF_EINVAL, "raster2dgs_bwd: null output");
     GSSDF_REQUIRE(a->isect_cap >= 0, GSSDF_EINVAL, "raster2dgs_bwd: negative isect_cap");
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_raster2dgs_bwd_workspace_bytes(a->C, a->image_width, a->image_height,
-                                                                                             a->cap, a->isect_cap),
-                  GSSDF_ENOMEM, "raster2dgs_bwd: workspace too small");
+    const RasterWs w = raster_ws(a->C, a->image_width, a->image_height, a->cap, a->isect_cap, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bwd_bytes, GSSDF_ENOMEM, "raster2dgs_bwd: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     const int tw = cdiv(a->image_width, kTile), th = cdiv(a->image_height, kTile);
-    const RasterWs w = carve_ws(a->workspace, a->C, a->image_width, a->image_height, a->cap, a->isect_cap);
     if (!a->reuse_fwd) {
         rc = pack_and_cull("raster2dgs_bwd", w, a->counts, a->C, a->image_width, a->image_height, a->cap, a->ray_transforms, a->colors,
                            a->opacities, a->normals, a->offsets, a->flatten_ids, nullptr, 0, st);

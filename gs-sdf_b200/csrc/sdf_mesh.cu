@@ -400,7 +400,7 @@ struct Ws {
     uint8_t *vinfo, *cases;
     float *ox, *osdf, *ones, *g3, *s7;
     void *cub;
-    size_t cub_bytes;
+    size_t cub_bytes, bytes;
 };
 
 bool make_plan(const gssdf_sdf_mesh_args *a, Plan *p) {
@@ -422,43 +422,37 @@ bool make_plan(const gssdf_sdf_mesh_args *a, Plan *p) {
     return true;
 }
 
-size_t layout(const gssdf_sdf_mesh_args *a, const Plan &p, void *base, Ws *w) {
-    size_t off = 0;
-    char *b = (char *)base;
-    auto take = [&](size_t bytes) {
-        char *q = b ? b + off : nullptr;
-        off = align_up(off + bytes, 256);
-        return (void *)q;
-    };
+Ws layout(const gssdf_sdf_mesh_args *a, const Plan &p, void *base) {
+    WsLayout L(base);
     Ws t;
     const size_t N = (size_t)p.N;
-    t.keys_in = (unsigned long long *)take(N * 8);
-    t.keys = (unsigned long long *)take(N * 8);
-    t.hk = (unsigned long long *)take(((size_t)1 << p.hbits) * 8);
-    t.hv = (int32_t *)take(((size_t)1 << p.hbits) * 4);
-    t.occ = (int32_t *)take(N * 4);
-    t.opos = (int32_t *)take(N * 4);
-    t.tk = (int32_t *)take(N * 4);
-    t.tbase = (int32_t *)take(N * 4);
-    t.rv = (int32_t *)take(N * 4);
-    t.vbase = (int32_t *)take(N * 4);
-    t.ref = (uint32_t *)take(N * 4);
-    t.vinfo = (uint8_t *)take(N);
-    t.cases = (uint8_t *)take(N);
-    t.ox = (float *)take((size_t)p.occ_cap * 12);
-    t.osdf = (float *)take((size_t)p.occ_cap * 4);
-    t.scal = (int32_t *)take(64);
+    t.keys_in = L.take<unsigned long long>(N);
+    t.keys = L.take<unsigned long long>(N);
+    t.hk = L.take<unsigned long long>((size_t)1 << p.hbits);
+    t.hv = L.take<int32_t>((size_t)1 << p.hbits);
+    t.occ = L.take<int32_t>(N);
+    t.opos = L.take<int32_t>(N);
+    t.tk = L.take<int32_t>(N);
+    t.tbase = L.take<int32_t>(N);
+    t.rv = L.take<int32_t>(N);
+    t.vbase = L.take<int32_t>(N);
+    t.ref = L.take<uint32_t>(N);
+    t.vinfo = L.take<uint8_t>(N);
+    t.cases = L.take<uint8_t>(N);
+    t.ox = L.take<float>((size_t)p.occ_cap * 3);
+    t.osdf = L.take<float>((size_t)p.occ_cap);
+    t.scal = L.take<int32_t>(16);
     const size_t vcap = (size_t)std::max<int64_t>(a->vertex_cap, 0);
-    t.ones = (float *)take(a->color_mode == 1 ? vcap * 4 : 0);
-    t.g3 = (float *)take(a->color_mode == 1 ? vcap * 12 : 0);
-    t.s7 = (float *)take(a->color_mode == 2 ? vcap * 28 : 0);
+    t.ones = L.take<float>(a->color_mode == 1 ? vcap : 0);
+    t.g3 = L.take<float>(a->color_mode == 1 ? vcap * 3 : 0);
+    t.s7 = L.take<float>(a->color_mode == 2 ? vcap * 7 : 0);
     size_t sort_b = 0, scan_b = 0;
     cub::DeviceRadixSort::SortKeys(nullptr, sort_b, (const unsigned long long *)nullptr, (unsigned long long *)nullptr, (int)p.N, 0, p.kbits);
     cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const int32_t *)nullptr, (int32_t *)nullptr, (int)p.N);
     t.cub_bytes = std::max(sort_b, scan_b);
-    t.cub = take(t.cub_bytes);
-    if (w) *w = t;
-    return off;
+    t.cub = L.take<char>(t.cub_bytes);
+    t.bytes = L.bytes();
+    return t;
 }
 
 }  // namespace
@@ -469,7 +463,7 @@ using namespace gssdf;
 extern "C" size_t gssdf_sdf_mesh_workspace_bytes(const gssdf_sdf_mesh_args *a) {
     Plan p;
     if (!a || !make_plan(a, &p) || 5 * p.N > INT32_MAX || a->n[0] <= 0 || a->n[1] <= 0 || a->n[2] <= 0) return 0;
-    return layout(a, p, nullptr, nullptr);
+    return layout(a, p, nullptr).bytes;
 }
 
 extern "C" int gssdf_sdf_mesh(const gssdf_sdf_mesh_args *a, gssdf_stream_t stream) {
@@ -498,14 +492,13 @@ extern "C" int gssdf_sdf_mesh(const gssdf_sdf_mesh_args *a, gssdf_stream_t strea
                   34);
     GSSDF_REQUIRE(5 * p.N <= INT32_MAX, GSSDF_EINVAL, "sdf_mesh: %lld leaves at this res may give more than 2^31 - 1 faces",
                   (long long)a->n_leaves);
-    const size_t need = layout(a, p, nullptr, nullptr);
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= need, GSSDF_ENOMEM, "sdf_mesh: workspace too small (%zu < %zu)", a->workspace_bytes, need);
+    const Ws w = layout(a, p, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "sdf_mesh: workspace too small (%zu < %zu)", a->workspace_bytes,
+                  w.bytes);
     cudaStream_t s = (cudaStream_t)stream;
     GSSDF_CUDA_OK(cudaMemsetAsync(a->counts, 0, 4 * sizeof(int32_t), s));
     if (a->n_leaves == 0) return GSSDF_OK;
 
-    Ws w;
-    layout(a, p, a->workspace, &w);
     Lattice L;
     for (int k = 0; k < 3; ++k) {
         L.n[k] = a->n[k];

@@ -389,12 +389,28 @@ static TileGeom make_geom(int W, int H, int tile_size) {
     return g;
 }
 
+struct TileWs {
+    int32_t *hist, *bin_start;
+    unsigned long long *keys;
+    int32_t *big;  // the three sort tiers' list lengths, then their bin lists
+    size_t bytes;
+};
+
+static TileWs tile_ws(int32_t C, const TileGeom &g, int64_t isect_cap, void *base) {
+    const size_t bins = (size_t)(C > 0 ? C : 1) * g.n_tiles;
+    WsLayout L(base);
+    TileWs w;
+    w.hist = L.take<int32_t>(bins);
+    w.bin_start = L.take<int32_t>(bins + 1);
+    w.keys = L.take<unsigned long long>(isect_cap > 0 ? isect_cap : 1);
+    w.big = L.take<int32_t>(3 * bins + 4);
+    w.bytes = L.bytes();
+    return w;
+}
+
 extern "C" size_t gssdf_tile_encode_workspace_bytes(int32_t C, int32_t W, int32_t H, int32_t tile_size, int64_t isect_cap) {
     if (tile_size <= 0) return 0;
-    const TileGeom g = make_geom(W, H, tile_size);
-    const size_t bins = (size_t)(C > 0 ? C : 1) * g.n_tiles;
-    return align_up(bins * 4, 256) + align_up((bins + 1) * 4, 256) + align_up((size_t)(isect_cap > 0 ? isect_cap : 1) * 8, 256) +
-           align_up((3 * bins + 4) * 4, 256);
+    return tile_ws(C, make_geom(W, H, tile_size), isect_cap, nullptr).bytes;
 }
 
 extern "C" int gssdf_tile_encode(const gssdf_tile_encode_args *a, gssdf_stream_t stream) {
@@ -407,19 +423,11 @@ extern "C" int gssdf_tile_encode(const gssdf_tile_encode_args *a, gssdf_stream_t
     while ((1u << cam_bits) <= (uint32_t)a->C) ++cam_bits;
     GSSDF_REQUIRE(g.tile_n_bits + cam_bits <= 32, GSSDF_EINVAL, "tile_encode: tile_n_bits + cam_n_bits > 32");
     const int bins = a->C * g.n_tiles;
-    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= gssdf_tile_encode_workspace_bytes(a->C, a->image_width,
-                                                                                         a->image_height, a->tile_size,
-                                                                                         a->isect_cap),
-                  GSSDF_ENOMEM, "tile_encode: workspace too small");
+    const TileWs w = tile_ws(a->C, g, a->isect_cap, a->workspace);
+    GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "tile_encode: workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = reinterpret_cast<char *>(a->workspace);
-    int32_t *hist = reinterpret_cast<int32_t *>(ws);
-    ws += align_up((size_t)bins * 4, 256);
-    int32_t *bin_start = reinterpret_cast<int32_t *>(ws);
-    ws += align_up((size_t)(bins + 1) * 4, 256);
-    unsigned long long *keys = reinterpret_cast<unsigned long long *>(ws);
-    ws += align_up((size_t)(a->isect_cap > 0 ? a->isect_cap : 1) * 8, 256);
-    int32_t *big = reinterpret_cast<int32_t *>(ws);
+    int32_t *hist = w.hist, *bin_start = w.bin_start, *big = w.big;
+    unsigned long long *keys = w.keys;
     constexpr int SS = 256, S0 = 2048, S1 = 8192, S2 = 28672;
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
