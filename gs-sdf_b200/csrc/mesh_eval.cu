@@ -10,14 +10,13 @@
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "morton.cuh"
 
 namespace gssdf {
 namespace {
 
 constexpr int kThreads = 256;
 constexpr int kMinBlocks = 1024;                     // fixed grid of the min-bound reduction (its partials live in the workspace)
-constexpr int kMortonBits = 21;                      // per axis: 63-bit keys
-constexpr uint64_t kSentinel = ~0ull;                // sorts after every 63-bit key
 constexpr int kPartial = 5;                          // per-block nearest-neighbour partials: kept, inliers, clamped, sum d, sum d^2
 constexpr double kTwo53Inv = 1.0 / 9007199254740992.0;
 
@@ -36,17 +35,6 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32
 __device__ __forceinline__ double u53(uint32_t hi, uint32_t lo) {
     return (double)(((uint64_t)(hi >> 5) << 26) | (uint64_t)(lo >> 6)) * kTwo53Inv;
 }
-
-__device__ __forceinline__ uint64_t spread3(uint32_t v) {  // bit b of v -> bit 3b
-    uint64_t x = v & 0x1fffffu;
-    x = (x | x << 32) & 0x1f00000000ffffull;
-    x = (x | x << 16) & 0x1f0000ff0000ffull;
-    x = (x | x << 8) & 0x100f00f00f00f00full;
-    x = (x | x << 4) & 0x10c30c30c30c30c3ull;
-    x = (x | x << 2) & 0x1249249249249249ull;
-    return x;
-}
-__device__ __forceinline__ uint64_t morton(uint32_t x, uint32_t y, uint32_t z) { return spread3(x) | spread3(y) << 1 | spread3(z) << 2; }
 
 struct Box {
     double c[3], R[9], h[3];  // centre, row-major rotation (column i = axis i), half extents

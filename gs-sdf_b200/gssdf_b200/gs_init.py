@@ -3,7 +3,10 @@
 `init_gs_with_sdf` is the reference's init_gs_with_sdf (include/neural_gaussian/neural_gaussian.cpp:19-127) as one gssdf_sdf_init_gs call;
 `neural_gs_init` is the tensor part of NeuralGS::NeuralGS's `mesh_init && sdf_enable && geo_init` branch (:273-424): mesh the SDF, stride
 the vertices down to the anchors, orient them from the SDF, append the sky sphere, draw the colours and drop NaN rows. The library never
-syncs or allocates; `neural_gs_init` reads the mesh counts and the NaN count back once each, like the reference."""
+syncs or allocates; `neural_gs_init` reads the mesh counts and the NaN count back once each, like the reference.
+
+f-10 (DESIGN 7k): `dist_cuda2` is simple-knn's distCUDA2 as one gssdf_knn3_mean_dist2 call, and `neural_gs_init_points` is the
+constructor's other branch, which starts from the depth cloud and sizes each splat by its three nearest neighbours."""
 import ctypes as C
 import math
 
@@ -96,13 +99,14 @@ def anchor_log_scale(mesh_res):
 
 
 def neural_gs_init(tree, net, margin_box, leaf_size, *, vis_batch_pt_num, sh_degree, spatial_scale, inner_map_size, map_origin, sky=True,
-                   generator=None):
+                   generator=None, geo_init=True, cpu_generator=None):
     """The tensors NeuralGS::NeuralGS builds on its `k_mesh_init && sdf_enable && k_geo_init` branch (neural_gaussian.cpp:293-424), in the
     reference's order:
       1. mesh.meshing(tree, net, *margin_box, 0.5 * leaf_size) -- its vertices are already the unique(faces) set (DESIGN 7f);
       2. anchors = the vertices strided by `anchor_indices` (the last vertex is excluded when striding, as in the reference);
          scaling = log(mesh_res);
-      3. quaternion / opacity from gssdf_sdf_init_gs (init_opa = true);
+      3. quaternion / opacity from gssdf_sdf_init_gs (init_opa = true); with geo_init=False (k_geo_init = 0) random_quat on
+         `cpu_generator` and opacity logit(0.1) instead;
       4. sky (k_sky_init): int(1000 * spatial_scale) points randn -> normalize(eps 1e-6) -> * 0.6 inner_map_size + map_origin, scale
          log(1.1 pi r^2 / n), quaternions from gssdf_rot6d_to_quat(samples, samples[:, (1, 2, 0)]), opacity logit(1) = +inf;
       5. offsets = 0, features_dc = rand [N,1,3], features_rest = 0 [N, (sh_degree+1)^2 - 1, 3];
@@ -118,22 +122,100 @@ def neural_gs_init(tree, net, margin_box, leaf_size, *, vis_batch_pt_num, sh_deg
     idx = anchor_indices(v.shape[0], vis_batch_pt_num)
     anchors = v[idx.start:idx.stop:idx.step].contiguous() if len(idx) else v[:0]
     scaling = torch.full((anchors.shape[0], 3), anchor_log_scale(mesh_res), dtype=torch.float32, device=dev)
-    r = init_gs_with_sdf(net, anchors, mesh_res, True)
-    quaternion, opacity = r["quaternion"], r["opacity"]
+    quaternion, opacity = _orientation(net if geo_init else None, anchors, mesh_res, cpu_generator)
     if sky:
-        n_sky = sky_count(spatial_scale)
-        radius = sky_radius(inner_map_size)
-        samples = torch.randn(n_sky, 3, dtype=torch.float32, device=dev, generator=generator)
-        samples = torch.nn.functional.normalize(samples, dim=-1, eps=1e-6)
-        origin = torch.as_tensor(np.asarray(map_origin, np.float32).reshape(1, 3), device=dev)
-        sky_anchor = samples * radius + origin
-        sky_scale = torch.full((n_sky, 3), sky_log_scale(inner_map_size, n_sky), dtype=torch.float32, device=dev)
-        sky_quat = rot6d_to_quat(samples, samples[:, [1, 2, 0]].contiguous())
-        sky_opacity = torch.logit(torch.ones(n_sky, dtype=torch.float32, device=dev))
-        anchors = torch.cat([anchors, sky_anchor], 0)
-        scaling = torch.cat([scaling, sky_scale], 0)
-        quaternion = torch.cat([quaternion, sky_quat], 0)
-        opacity = torch.cat([opacity, sky_opacity], 0)
+        anchors, scaling, quaternion, opacity = append_sky(anchors, scaling, quaternion, opacity, spatial_scale, inner_map_size, map_origin,
+                                                           generator)
+    return finish_rows(anchors, scaling, quaternion, opacity, sh_degree, generator)
+
+
+def _orientation(net, anchors, mesh_res, cpu_generator):
+    """quaternion and opacity of NeuralGS::NeuralGS (neural_gaussian.cpp:321-333): from gssdf_sdf_init_gs with init_opa when the SDF is
+    enabled and k_geo_init is set (net given), else random_quat on the CPU generator and logit(0.1f)."""
+    if net is not None:
+        r = init_gs_with_sdf(net, anchors, mesh_res, True)
+        return r["quaternion"], r["opacity"]
+    n, dev = anchors.shape[0], anchors.device
+    return random_quat(n, cpu_generator).to(dev), torch.logit(0.1 * torch.ones(n, dtype=torch.float32, device=dev))
+
+
+def append_sky(anchors, scaling, quaternion, opacity, spatial_scale, inner_map_size, map_origin, generator=None):
+    """Step 4 of neural_gs_init (k_sky_init, neural_gaussian.cpp:335-401): int(1000 * spatial_scale) points randn (from `generator`) ->
+    normalize(eps 1e-6) -> * 0.6 inner_map_size + map_origin, scale log(1.1 pi r^2 / n), quaternions from gssdf_rot6d_to_quat(samples,
+    samples[:, (1, 2, 0)]), opacity logit(1) = +inf; appended after the given rows. Returns (anchors, scaling, quaternion, opacity)."""
+    dev = anchors.device
+    n_sky = sky_count(spatial_scale)
+    radius = sky_radius(inner_map_size)
+    samples = torch.randn(n_sky, 3, dtype=torch.float32, device=dev, generator=generator)
+    samples = torch.nn.functional.normalize(samples, dim=-1, eps=1e-6)
+    origin = torch.as_tensor(np.asarray(map_origin, np.float32).reshape(1, 3), device=dev)
+    sky_anchor = samples * radius + origin
+    sky_scale = torch.full((n_sky, 3), sky_log_scale(inner_map_size, n_sky), dtype=torch.float32, device=dev)
+    sky_quat = rot6d_to_quat(samples, samples[:, [1, 2, 0]].contiguous())
+    sky_opacity = torch.logit(torch.ones(n_sky, dtype=torch.float32, device=dev))
+    return (torch.cat([anchors, sky_anchor], 0), torch.cat([scaling, sky_scale], 0), torch.cat([quaternion, sky_quat], 0),
+            torch.cat([opacity, sky_opacity], 0))
+
+
+def knn3_mean_dist2(points, out, ws=None):
+    """Raw gssdf_knn3_mean_dist2 on a caller-allocated output (points CUDA float32 [n,3] contiguous, out float32 [n])."""
+    n = points.shape[0]
+    ws = ws or cabi.Workspace(points.device)
+    w = ws.get(lib().gssdf_knn3_mean_dist2_workspace_bytes(n))
+    a = make_args("gssdf_knn3_mean_dist2_args", n=n, points=points, out=out, workspace=w, workspace_bytes=w.numel())
+    check(lib().gssdf_knn3_mean_dist2(C.byref(a), cabi._stream()))
+    return out
+
+
+def dist_cuda2(points, ws=None):
+    """simple-knn's distCUDA2(points) (submodules/simple-knn/spatial.cu): for each point the mean of its three smallest squared distances
+    to the other points, float32 [P] on the points' device (include/gssdf_b200.h f-10, DESIGN 7k). points: CUDA float32 [P,3], made
+    contiguous as the reference does."""
+    if not isinstance(points, torch.Tensor) or points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"gssdf_b200: points must be a [P,3] tensor, got {tuple(getattr(points, 'shape', ()))}")
+    x = cabi._req(points.contiguous(), torch.float32, "points")
+    return knn3_mean_dist2(x, torch.empty(x.shape[0], dtype=torch.float32, device=x.device), ws)
+
+
+def init_point_indices(n_points):
+    """The reference's stride of the depth cloud before NeuralGS (neural_mapping.cpp:843-848): step = int(N / 1e6f) in fp32 (N rounded
+    to fp32 first), at least 1, and slice(0, 0, -1, step) -- which always stops before the LAST point. Returns a Python range."""
+    step = max(int(_f32(_f32(n_points) / _f32(1e6))), 1)
+    return range(0, max(n_points - 1, 0), step)
+
+
+def random_quat(n, cpu_generator=None):
+    """random_quat_tensor(N) (include/neural_gaussian/gauss_utils.hpp:32-46): u, v, w = three torch.rand(N) draws from the CPU generator,
+    q = (sqrt(1 - u) sin(2 pi v), sqrt(1 - u) cos(2 pi v), sqrt(u) sin(2 pi w), sqrt(u) cos(2 pi w)) in fp32 (2 pi rounded to fp32 by
+    ATen's scalar multiply). Returns a CPU float32 [n,4] tensor; NeuralGS moves it to the device."""
+    u = torch.rand(n, generator=cpu_generator)
+    v = torch.rand(n, generator=cpu_generator)
+    w = torch.rand(n, generator=cpu_generator)
+    return torch.stack([torch.sqrt(1 - u) * torch.sin(2 * math.pi * v), torch.sqrt(1 - u) * torch.cos(2 * math.pi * v),
+                        torch.sqrt(u) * torch.sin(2 * math.pi * w), torch.sqrt(u) * torch.cos(2 * math.pi * w)], -1)
+
+
+def neural_gs_init_points(points, *, net=None, leaf_size, geo_init=True, sh_degree, spatial_scale, inner_map_size, map_origin, sky=True,
+                          generator=None, cpu_generator=None):
+    """The tensors NeuralGS::NeuralGS builds when it starts from points rather than from the SDF mesh (k_mesh_init = 0 or the SDF
+    disabled; neural_gaussian.cpp:312-424), in the reference's order:
+      1. anchors = points (the caller's depth cloud, strided by `init_point_indices` in the reference's trainer);
+         scaling = log(sqrt(clamp_min(dist_cuda2(points), 1e-6))) repeated over the three axes;
+      2. with an SDF (`net`) and geo_init: quaternion / opacity from gssdf_sdf_init_gs at delta 0.5 * leaf_size (init_opa = true);
+         otherwise random_quat(n, cpu_generator) and opacity logit(0.1);
+      3. the sky (k_sky_init), features and NaN-row filter exactly as neural_gs_init (append_sky, finish_rows).
+    Random draws in the reference's order: the CPU u, v, w of random_quat, then `generator`'s sky randn and features_dc rand.
+    Returns (dict, number of dropped NaN rows) like neural_gs_init."""
+    anchors = cabi._req(points, torch.float32, "points")
+    if anchors.dim() != 2 or anchors.shape[1] != 3:
+        raise ValueError(f"gssdf_b200: points must be [n,3], got {tuple(anchors.shape)}")
+    dist2 = torch.clamp_min(dist_cuda2(anchors), 1e-6)
+    scaling = torch.log(torch.sqrt(dist2)).unsqueeze(-1).repeat(1, 3)
+    mesh_res = float(_f32(_f32(0.5) * _f32(leaf_size)))
+    quaternion, opacity = _orientation(net if geo_init else None, anchors, mesh_res, cpu_generator)
+    if sky:
+        anchors, scaling, quaternion, opacity = append_sky(anchors, scaling, quaternion, opacity, spatial_scale, inner_map_size, map_origin,
+                                                           generator)
     return finish_rows(anchors, scaling, quaternion, opacity, sh_degree, generator)
 
 

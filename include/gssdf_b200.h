@@ -1204,6 +1204,33 @@ typedef struct gssdf_nn_truncated_args {
 size_t gssdf_nn_truncated_workspace_bytes(int64_t cap_queries);
 int gssdf_nn_truncated(const gssdf_nn_truncated_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-10  Mean squared distance to the three nearest neighbours.  Replaces simple-knn's distCUDA2 (submodules/simple-knn/spatial.cu),
+ *     which NeuralGS::NeuralGS (include/neural_gaussian/neural_gaussian.cpp:312-318) calls on the strided depth cloud to size the initial
+ *     splats when they do not start from the SDF mesh (DESIGN 7k). One call, no allocation, no sync; all arguments are checked before the
+ *     first launch; bit-identical from run to run and capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+/* For each point i of points [n,3] (fp32):
+     out[i] = ((b0 + b1) + b2) / 3     (fp32, each operation one IEEE rounding)
+   where b0 <= b1 <= b2 are the three smallest d2(i, j) over j != i (a distinct index: a duplicate point contributes 0) with
+   d2 < FLT_MAX, missing entries counting as FLT_MAX, and
+     d2(i, j) = fma(dz, dz, fma(dx, dx, dy * dy)),   d = p_j - p_i per axis in fp32
+   (the contraction nvcc gives simple-knn's distance sums in the reference's build: the y term is the product). So n = 1 or 2 gives +inf, n = 3 gives fl(fl(b0 + b1) + FLT_MAX) / 3
+   (about 1.13e38), and a point with a NaN or infinite coordinate never enters another point's list and gets +inf itself. The result
+   depends on the point set only, not on the order of the rows; it equals distCUDA2's for every input that distCUDA2 accepts.
+   GSSDF_EINVAL before any launch for n outside [0, 2^31), a NULL points, out or workspace when n > 0, or a workspace that is too small.
+   n == 0 is a no-op. */
+typedef struct gssdf_knn3_mean_dist2_args {
+    int64_t n;
+    const float *points;          /* [n,3] */
+    float *out;                   /* [n] */
+    void *workspace;              /* >= gssdf_knn3_mean_dist2_workspace_bytes(n) */
+    size_t workspace_bytes;
+} gssdf_knn3_mean_dist2_args;
+/* 0 for n outside [0, 2^31) */
+size_t gssdf_knn3_mean_dist2_workspace_bytes(int64_t n);
+int gssdf_knn3_mean_dist2(const gssdf_knn3_mean_dist2_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
