@@ -315,30 +315,31 @@ raster2dgs_fwd_kernel(const gssdf_raster2dgs_fwd_args a, const float4 *__restric
 // into its own partial row; the batch flush sums the four rows. No shared-memory float atomics (sm_90 has none: they would be CAS loops).
 constexpr int kBwdThreads = 128;
 constexpr int kBwdWarps = kBwdThreads / 32;
-constexpr int kBwdBatch = 64;     // splats per shared-memory stage: 2 stages = 41 KiB -> 5 CTAs (20 warps) per SM
-constexpr int kBwdMinBlocks = 5;  // CTAs per SM the register allocation is held to
+constexpr int kBwdBatch = 64;     // splats per shared-memory stage: 2 stages + one partial buffer = 26 KiB
+constexpr int kBwdMinBlocks = 6;  // CTAs per SM the register allocation is held to: 80 registers, no spills
 
-template <bool ABS>
-struct __align__(16) BwdStageT {
+// the record ring: two stages, refilled by TMA while the other is walked
+struct __align__(16) BwdStage {
     float4 rec[kBwdBatch * kRecF4];
-    float part[kBwdWarps * kBwdBatch * 16];            // [warp][slot][16] reduced gradient records: rgb[3] n[3] u[3] v[3] w[3] opacity
-    float gabs[ABS ? kBwdWarps * 2 * kBwdBatch : 4];  // [warp][u.z | v.z][slot] absgrad partials
     int ids[kBwdBatch];
     int meta[kBwdBatch];
 };
 
+// the warps' reduced gradient records of the batch being walked. One buffer serves both stages: the flush reads it between the two
+// batch barriers and zeroes what it read, so it is clean again before any warp walks the next batch.
 template <bool ABS>
-__device__ __forceinline__ void issue_batch_bwd(BwdStageT<ABS> &st, uint64_t *bar, const float4 *__restrict__ rec,
+struct __align__(16) BwdPartT {
+    float part[kBwdWarps * kBwdBatch * 16];            // [warp][slot][16] reduced gradient records: rgb[3] n[3] u[3] v[3] w[3] opacity
+    float gabs[ABS ? kBwdWarps * 2 * kBwdBatch : 4];  // [warp][u.z | v.z][slot] absgrad partials
+};
+
+template <bool ABS>
+constexpr size_t bwd_smem_bytes() { return 2 * sizeof(BwdStage) + sizeof(BwdPartT<ABS>); }
+
+__device__ __forceinline__ void issue_batch_bwd(BwdStage &st, uint64_t *bar, const float4 *__restrict__ rec,
                                                 const int2 *__restrict__ clist, int last, int n) {
     // batch covers culled-list entries last, last-1, ..., last-n+1 (slot t <-> entry last - t): back to front
     const int t = threadIdx.x;
-    float4 *part4 = reinterpret_cast<float4 *>(st.part);
-#pragma unroll
-    for (int k = t; k < kBwdWarps * kBwdBatch * 4; k += kBwdThreads) part4[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (ABS) {
-#pragma unroll
-        for (int k = t; k < kBwdWarps * 2 * kBwdBatch; k += kBwdThreads) st.gabs[k] = 0.f;
-    }
     if (t < n) {
         const int2 e = clist[last - t];
         st.ids[t] = e.x;
@@ -350,11 +351,12 @@ __device__ __forceinline__ void issue_batch_bwd(BwdStageT<ABS> &st, uint64_t *ba
     }
 }
 
-// per-pixel state of the backward walk: transmittance, the colour / normal / depth composited behind the current splat, the cotangents
+// per-pixel state of the backward walk: transmittance, R = va - (colour, normal, depth composited behind the current splat) . (their
+// cotangents), the cotangents. The reference keeps the seven sums behind the splat and dots them with the cotangents at every step; only
+// that dot product enters the VJP, so one running sum of fac * (record . cotangents) replaces them.
 struct BwdPixel {
-    float T;
-    float bc0, bc1, bc2, bn0, bn1, bn2, bd;
-    float vc0, vc1, vc2, vd, va, vn0, vn1, vn2, v_median;  // va: T_final * (alpha cotangent - background . colour cotangent)
+    float T, R;  // R starts at va = T_final * (alpha cotangent - background . colour cotangent)
+    float vc0, vc1, vc2, vd, vn0, vn1, vn2, v_median;
     int bin_final, median_idx;  // -1 outside the image: no splat index is <= -1
 };
 
@@ -364,29 +366,27 @@ __device__ __forceinline__ void bwd_pixel_init(BwdPixel &P, const gssdf_raster2d
     const bool inside = i < H && j < W;
     const int64_t pix = inside ? ((int64_t)ti.cam * H + i) * W + j : 0;
     P.T = inside ? 1.f - a.render_alphas[pix] : 1.f;  // T_final
-    P.bc0 = P.bc1 = P.bc2 = P.bn0 = P.bn1 = P.bn2 = P.bd = 0.f;
     // pixels that never composited anything keep last_ids == 0 (Fwd.cu:209,463); index 0 only
     // exists in the first non-empty tile, elsewhere nothing is <= bin_final.
     P.bin_final = inside ? a.last_ids[pix] : -1;
     P.median_idx = inside ? a.median_ids[pix] : -1;
-    P.vc0 = P.vc1 = P.vc2 = P.vd = P.va = P.vn0 = P.vn1 = P.vn2 = P.v_median = 0.f;
+    P.vc0 = P.vc1 = P.vc2 = P.vd = P.R = P.vn0 = P.vn1 = P.vn2 = P.v_median = 0.f;
     if (inside) {
         P.vc0 = a.v_render_colors[3 * pix]; P.vc1 = a.v_render_colors[3 * pix + 1]; P.vc2 = a.v_render_colors[3 * pix + 2];
         P.vd = a.v_render_depths[pix];
-        P.va = a.v_render_alphas[pix];
+        P.R = a.v_render_alphas[pix];
         P.vn0 = a.v_render_normals[3 * pix]; P.vn1 = a.v_render_normals[3 * pix + 1]; P.vn2 = a.v_render_normals[3 * pix + 2];
         P.v_median = a.v_render_median[pix];
     }
     if (a.backgrounds)
-        P.va -= a.backgrounds[3 * ti.cam] * P.vc0 + a.backgrounds[3 * ti.cam + 1] * P.vc1 + a.backgrounds[3 * ti.cam + 2] * P.vc2;
-    P.va *= P.T;
+        P.R -= a.backgrounds[3 * ti.cam] * P.vc0 + a.backgrounds[3 * ti.cam + 1] * P.vc1 + a.backgrounds[3 * ti.cam + 2] * P.vc2;
+    P.R *= P.T;
 }
 
 // one (pixel, splat) step of the back-to-front walk: the reference's per-pixel VJP (Bwd.cu), added into g[16]; returns whether the splat
-// contributed to this pixel
-__device__ __forceinline__ bool bwd_pixel_splat(BwdPixel &P, float px, float py, int idx, const float4 r0, const float4 r1, const float4 r2,
-                                                const float4 r3, float g[16]) {
-    const float hux = px * r1.z - r0.x, huy = px * r1.w - r0.y, huz = px * r2.x - r0.z;
+// contributed to this pixel. h_u = px * M_w - M_u depends on the pixel's column only: the caller computes it once for both halves.
+__device__ __forceinline__ bool bwd_pixel_splat(BwdPixel &P, float px, float py, float hux, float huy, float huz, int idx, const float4 r0,
+                                                const float4 r1, const float4 r2, const float4 r3, float g[16]) {
     const float hvx = py * r1.z - r0.w, hvy = py * r1.w - r1.x, hvz = py * r2.x - r1.y;
     const float rcx = huy * hvz - huz * hvy, rcy = huz * hvx - hux * hvz, rcz = hux * hvy - huy * hvx;
     bool valid = idx <= P.bin_final && rcz != 0.f;
@@ -407,10 +407,10 @@ __device__ __forceinline__ bool bwd_pixel_splat(BwdPixel &P, float px, float py,
         const float fac = alpha * T;
         g[0] += fac * P.vc0; g[1] += fac * P.vc1; g[2] += fac * P.vc2;
         g[3] += fac * P.vn0; g[4] += fac * P.vn1; g[5] += fac * P.vn2;
-        float v_alpha = (r2.z * T - P.bc0 * ra) * P.vc0 + (r2.w * T - P.bc1 * ra) * P.vc1 + (r3.x * T - P.bc2 * ra) * P.vc2;
-        v_alpha += (r3.y * T - P.bn0 * ra) * P.vn0 + (r3.z * T - P.bn1 * ra) * P.vn1 + (r3.w * T - P.bn2 * ra) * P.vn2;
-        v_alpha += ra * P.va;
-        v_alpha += (depth * T - P.bd * ra) * P.vd;
+        // d = (colour, normal, depth of this splat) . cotangents; the reference's sum over the seven channels of
+        // (value * T - behind * ra) * cotangent, plus ra * va, is T * d + ra * R
+        const float d = (r2.z * P.vc0 + r2.w * P.vc1 + r3.x * P.vc2) + (r3.y * P.vn0 + r3.z * P.vn1 + r3.w * P.vn2) + depth * P.vd;
+        const float v_alpha = T * d + ra * P.R;
         if (opac * vis <= 0.999f) {
             v_depth += fac * P.vd;
             const float v_G = opac * v_alpha;
@@ -428,9 +428,7 @@ __device__ __forceinline__ bool bwd_pixel_splat(BwdPixel &P, float px, float py,
             g[14] += px * vhuz + py * vhvz + v_depth;
             g[15] += vis * v_alpha;
         }
-        P.bc0 += r2.z * fac; P.bc1 += r2.w * fac; P.bc2 += r3.x * fac;
-        P.bd += depth * fac;
-        P.bn0 += r3.y * fac; P.bn1 += r3.z * fac; P.bn2 += r3.w * fac;
+        P.R -= fac * d;
     }
     return valid;
 }
@@ -439,9 +437,9 @@ template <bool ABS>
 __global__ void __launch_bounds__(kBwdThreads, kBwdMinBlocks)
 raster2dgs_bwd_kernel(const gssdf_raster2dgs_bwd_args a, const float4 *__restrict__ rec, const int2 *__restrict__ clist,
                       const int32_t *__restrict__ ccount, float *__restrict__ vrec, int tw, int th) {
-    using BwdStage = BwdStageT<ABS>;
     extern __shared__ __align__(16) unsigned char s_raw[];
     BwdStage *s_stage = reinterpret_cast<BwdStage *>(s_raw);
+    BwdPartT<ABS> &s_part = *reinterpret_cast<BwdPartT<ABS> *>(s_raw + 2 * sizeof(BwdStage));
     __shared__ __align__(8) uint64_t s_bar[2];
     const TileInfo ti = tile_info(a.C, tw, th, a.offsets, a.counts);
     const int n_total = ccount[blockIdx.x];  // culled list length
@@ -456,6 +454,12 @@ raster2dgs_bwd_kernel(const gssdf_raster2dgs_bwd_args a, const float4 *__restric
         mbar_init(&s_bar[0], kBwdThreads);
         mbar_init(&s_bar[1], kBwdThreads);
         fence_mbar_init();
+    }
+    {
+        float4 *part4 = reinterpret_cast<float4 *>(s_part.part);
+        for (int k = threadIdx.x; k < kBwdWarps * kBwdBatch * 4; k += kBwdThreads) part4[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (ABS)
+            for (int k = threadIdx.x; k < kBwdWarps * 2 * kBwdBatch; k += kBwdThreads) s_part.gabs[k] = 0.f;
     }
     __syncthreads();
 
@@ -474,7 +478,7 @@ raster2dgs_bwd_kernel(const gssdf_raster2dgs_bwd_args a, const float4 *__restric
         mbar_wait(&s_bar[b & 1], (b >> 1) & 1);
         const int last = c_last - b * kBwdBatch;  // culled-list entry held by slot 0
         const int bn = min(kBwdBatch, last - ti.rs + 1);
-        float *part = st.part + warp * kBwdBatch * 16;
+        float *part = s_part.part + warp * kBwdBatch * 16;
         for (int t0 = 0; t0 < bn; t0 += 32) {
           const int my_meta = (t0 + lane < bn) ? st.meta[t0 + lane] : 0;
           // skip the entries behind every pixel of this warp's last contributor (Bwd.cu:333) and those culled for both halves
@@ -490,9 +494,10 @@ raster2dgs_bwd_kernel(const gssdf_raster2dgs_bwd_args a, const float4 *__restric
 #pragma unroll
             for (int k = 0; k < 16; ++k) g[k] = 0.f;
             // warp-uniform: a half whose mask bit is clear holds no pixel the splat reaches (alpha < 1/255 there)
+            const float hux = px * r1.z - r0.x, huy = px * r1.w - r0.y, huz = px * r2.x - r0.z;
             bool any = false;
-            if ((m >> wb) & 1) any = bwd_pixel_splat(P0, px, py, idx, r0, r1, r2, r3, g);
-            if ((m >> (wb + 2)) & 1) any |= bwd_pixel_splat(P1, px, py + 4.f, idx, r0, r1, r2, r3, g);
+            if ((m >> wb) & 1) any = bwd_pixel_splat(P0, px, py, hux, huy, huz, idx, r0, r1, r2, r3, g);
+            if ((m >> (wb + 2)) & 1) any |= bwd_pixel_splat(P1, px, py + 4.f, hux, huy, huz, idx, r0, r1, r2, r3, g);
             if (!__any_sync(0xffffffffu, any)) continue;
 
             // butterfly reduction of the 16-float record over the 32 lanes: 8+4+2+1+1 shuffles
@@ -522,19 +527,22 @@ raster2dgs_bwd_kernel(const gssdf_raster2dgs_bwd_args a, const float4 *__restric
             if ((lane & 1) == 0) part[t * 16 + comp] = h1;  // this warp's row: 16 consecutive words, conflict-free
             if (ABS) {
                 // |sum over the warp's 8x8 pixel block of dL/dM_u.z (resp. M_v.z)| * M_w.z
-                if (lane == 16) st.gabs[(2 * warp) * kBwdBatch + t] = fabsf(h1 * r2.x);      // comp 8  = u.z
-                if (lane == 22) st.gabs[(2 * warp + 1) * kBwdBatch + t] = fabsf(h1 * r2.x);  // comp 11 = v.z
+                if (lane == 16) s_part.gabs[(2 * warp) * kBwdBatch + t] = fabsf(h1 * r2.x);      // comp 8  = u.z
+                if (lane == 22) s_part.gabs[(2 * warp + 1) * kBwdBatch + t] = fabsf(h1 * r2.x);  // comp 11 = v.z
             }
           }
         }
         __syncthreads();
-        // flush: sum the warps' rows, one 64-byte burst of four 16-byte REDs per (tile, splat); 4 consecutive threads cover one record
-        const float4 *part4 = reinterpret_cast<const float4 *>(st.part);
+        // flush: sum the warps' rows, one 64-byte burst of four 16-byte REDs per (tile, splat); 4 consecutive threads cover one record.
+        // Only slots < bn can have been written; each is zeroed by the thread that read it.
+        float4 *part4 = reinterpret_cast<float4 *>(s_part.part);
         for (int e = threadIdx.x; e < bn * 4; e += kBwdThreads) {
             float4 v = part4[e];
+            part4[e] = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int w = 1; w < kBwdWarps; ++w) {
                 const float4 p = part4[w * kBwdBatch * 4 + e];
+                part4[w * kBwdBatch * 4 + e] = make_float4(0.f, 0.f, 0.f, 0.f);
                 v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w;
             }
             if (v.x != 0.f || v.y != 0.f || v.z != 0.f || v.w != 0.f)
@@ -545,7 +553,10 @@ raster2dgs_bwd_kernel(const gssdf_raster2dgs_bwd_args a, const float4 *__restric
                 const int t = e >> 1, k = e & 1;
                 float v = 0.f;
 #pragma unroll
-                for (int w = 0; w < kBwdWarps; ++w) v += st.gabs[(2 * w + k) * kBwdBatch + t];
+                for (int w = 0; w < kBwdWarps; ++w) {
+                    v += s_part.gabs[(2 * w + k) * kBwdBatch + t];
+                    s_part.gabs[(2 * w + k) * kBwdBatch + t] = 0.f;
+                }
                 if (v != 0.f) atomicAdd(a.v_means2d_abs + 2 * (int64_t)st.ids[t] + k, v);
             }
         }
@@ -799,8 +810,8 @@ extern "C" int gssdf_raster2dgs_bwd(const gssdf_raster2dgs_bwd_args *a, gssdf_st
         kern<<<a->C * tw * th, kBwdThreads, smem, st>>>(*a, w.rec, w.clist, w.ccount, reinterpret_cast<float *>(w.vrec), tw, th);
         return GSSDF_OK;
     };
-    rc = a->v_means2d_abs ? launch(raster2dgs_bwd_kernel<true>, 2 * sizeof(BwdStageT<true>))
-                          : launch(raster2dgs_bwd_kernel<false>, 2 * sizeof(BwdStageT<false>));
+    rc = a->v_means2d_abs ? launch(raster2dgs_bwd_kernel<true>, bwd_smem_bytes<true>())
+                          : launch(raster2dgs_bwd_kernel<false>, bwd_smem_bytes<false>());
     if (rc) return rc;
     GSSDF_LAUNCH_OK("raster2dgs_bwd_kernel");
     if (a->prof_stop) GSSDF_CUDA_OK(cudaEventRecord((cudaEvent_t)a->prof_stop, st));
