@@ -8,6 +8,7 @@
 #include "cumcubes.hpp"
 #include "gssdf_init.hpp"
 #include "gssdf_mesh.hpp"
+#include "gssdf_metrics.hpp"
 #include "gssdf_octree.hpp"
 #include "spatial.h"
 
@@ -57,6 +58,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     });
     m.def("gssdf_cull_mesh_faces", &gssdf::cull_mesh_faces);
     m.def("gssdf_eval_mesh", &gssdf::eval_mesh);
+    m.def("gssdf_psnr", &gssdf::psnr);
+    m.def("gssdf_image_metrics", &gssdf::image_metrics, pybind11::arg("renders"), pybind11::arg("gts"), pybind11::arg("input_mode") = 2);
+    m.def("gssdf_eval_render", &gssdf::eval_render, pybind11::arg("renders"), pybind11::arg("gts"), pybind11::arg("names"),
+          pybind11::arg("chunk") = 64, pybind11::arg("input_mode") = 2);
     m.def("gssdf_update_octree_as", &gssdf::update_octree_as);
     m.def("distCUDA2", &distCUDA2);
     m.def("fully_fused_projection_2dgs", &fully_fused_projection_2dgs);

@@ -1231,6 +1231,50 @@ typedef struct gssdf_knn3_mean_dist2_args {
 size_t gssdf_knn3_mean_dist2_workspace_bytes(int64_t n);
 int gssdf_knn3_mean_dist2(const gssdf_knn3_mean_dist2_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-11  Image metrics of rendered views.  Replaces eval/image_metrics/metrics.py (PSNR and SSIM, without LPIPS), which
+ *     NeuralSLAM::eval_render (include/neural_mapping/neural_mapping.cpp:1435-1462) runs on the render directories, and the
+ *     loss_utils::psnr of export_test_image (:1202-1328) and prefilter_data (:595-669) (DESIGN 7l). One call scores V views; it never
+ *     allocates or syncs, checks every argument before the first launch and captures into a CUDA graph. Every `_rn` below is one IEEE
+ *     rounding (no contraction).
+ * ------------------------------------------------------------------------------------------ */
+/* Element c of pixel (x, y) of view v of an input is p[v * view_stride + (y * W + x) * pixel_stride + c], c = 0..2 (pixel_stride >= 3
+   elements, view_stride >= 0: 0 scores every view against the same image). Its value:
+     uint8 u                       fl_rn(u / 255)                              (to_tensor of an 8-bit PNG)
+     fp32 x, input_mode 0          x
+     fp32 x, input_mode 1          clamp(x, 0, 1)                              (export_test_image's render_color.clamp(0, 1))
+     fp32 x, input_mode 2          q = (uint8)(int64) fl_rn(clamp(x, 0, 1) * 255) (truncation; utils::tensor_to_cv_mat), then fl_rn(q / 255)
+   clamp passes NaN through, as torch's does; in mode 2 the cast then gives q = 0, as torch's CUDA .to(torch.uint8) does.
+   PSNR (image_utils.psnr / loss_utils::psnr): d = fl_rn(x - y), sse = the fp64 sum of fl_rn(d * d) over the 3 H W elements,
+     mse = sse / (3 H W), psnr = 20 log10(1 / sqrt(mse)) in fp64 (+inf when mse == 0).
+   SSIM (eval/image_metrics/loss_utils.py:45-86, size_average): the 1-D window g_i = exp(-(i - 5)^2 / 4.5), i = 0..10, in fp64, rounded
+     to fp32 and divided by the fp32 rounding of their fp64 sum (what torch's sum of the eleven fp32 values gives); the five maps x, y, fl(x x), fl(y y), fl(x y) are filtered separably
+     with zero padding 5, first along the row then along the column, each tap sum h = fl(h + fl(g_i v)) in i order;
+     with C1 = fl32(0.01^2), C2 = fl32(0.03^2) and every step in fp32:
+       S = ((2 mu_xy + C1)(2 s_xy + C2)) / (((mu_x^2 + mu_y^2) + C1)((s_x + s_y) + C2)),  s_x = E[x^2] - mu_x^2, s_xy = E[xy] - mu_x mu_y,
+     ssim_sum = the fp64 sum of S over the 3 H W elements, ssim = ssim_sum / (3 H W).
+   The fp64 sums are fixed trees: one partial per (view, channel, band of rows, strip of 32 columns) in its own workspace slot, reduced
+   per view by a second launch in a fixed order; the bands depend on W and H only. So results are bit-identical from run to run and
+   between one call of V views and V calls of one view. out (device double[V][4], overwritten): {sse, ssim_sum, psnr, ssim}.
+   GSSDF_EINVAL before any launch for V outside [0, 21845], W or H < 1, W H > 2^31, a dtype other than 0 / 1, a pixel stride below 3, a negative view
+   stride, input_mode outside 0..2, a required NULL pointer, or a workspace that is too small. V == 0 is a no-op. */
+typedef struct gssdf_image_metrics_args {
+    int32_t V, W, H;
+    const void *render;
+    int32_t render_dtype;         /* 0: float32, 1: uint8 */
+    int64_t render_pixel_stride, render_view_stride;  /* in elements */
+    const void *gt;
+    int32_t gt_dtype;             /* 0: float32, 1: uint8 */
+    int64_t gt_pixel_stride, gt_view_stride;
+    int32_t input_mode;           /* 0, 1, 2: applied to the fp32 inputs */
+    double *out;                  /* [V][4] */
+    void *workspace;              /* >= gssdf_image_metrics_workspace_bytes(V, W, H) */
+    size_t workspace_bytes;
+} gssdf_image_metrics_args;
+/* 0 for V outside [0, 21845], W or H < 1 or W H > 2^31 */
+size_t gssdf_image_metrics_workspace_bytes(int32_t V, int32_t W, int32_t H);
+int gssdf_image_metrics(const gssdf_image_metrics_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
