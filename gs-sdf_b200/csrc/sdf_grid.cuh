@@ -56,6 +56,21 @@ __device__ __forceinline__ uint32_t grid_index(uint32_t hashmap_size, uint32_t r
     return index;
 }
 
+// grid_index without branches: the same value, computed on both paths and selected. Branches end a basic block, and ptxas does not
+// move a load across one, so with grid_index a thread's gathers go out 8 at a time (one (point, level)); with this one a batch of
+// (point, level) tasks is straight-line code and all its gathers are in flight together.
+__device__ __forceinline__ uint32_t grid_index_sel(uint32_t hashmap_size, uint32_t res, uint32_t x, uint32_t y, uint32_t z) {
+    uint32_t stride = 1, index = 0;
+    bool s = stride <= hashmap_size;
+    index += s ? x * stride : 0u; stride = s ? stride * res : stride;
+    s = stride <= hashmap_size;
+    index += s ? y * stride : 0u; stride = s ? stride * res : stride;
+    s = stride <= hashmap_size;
+    index += s ? z * stride : 0u; stride = s ? stride * res : stride;
+    const uint32_t hashed = (x ^ (y * 2654435761u) ^ (z * 805459861u)) & (hashmap_size - 1u);
+    return hashmap_size < stride ? hashed : index % hashmap_size;  // index % hs == index whenever grid_index skips the division
+}
+
 struct LevelPos {
     float pos[3];
     uint32_t pg[3];
@@ -73,7 +88,9 @@ __device__ __forceinline__ LevelPos level_pos(const float x[3], float scale) {  
     return p;
 }
 
-// one (point, level): the two features, accumulated exactly like kernel_grid<__half>: result = hfma2((half)w, val, result)
+// one (point, level): the two features, accumulated exactly like kernel_grid<__half>: result = hfma2((half)w, val, result).
+// BRANCH_FREE: the corner indices come from grid_index_sel (same values), for callers that batch several tasks' gathers.
+template <bool BRANCH_FREE = false>
 __device__ __forceinline__ float2 encode_level(const __half2 *__restrict__ table, const GridGeom &g, int lvl, const float x[3]) {
     const __half2 *t = table + g.offset[lvl];
     const uint32_t hs = g.offset[lvl + 1] - g.offset[lvl];
@@ -90,7 +107,7 @@ __device__ __forceinline__ float2 encode_level(const __half2 *__restrict__ table
             else { wt *= p.pos[d]; c[d] = p.pg[d] + 1; }
         }
         w[idx] = wt;
-        vals[idx] = __ldg(t + grid_index(hs, g.res[lvl], c[0], c[1], c[2]));
+        vals[idx] = __ldg(t + (BRANCH_FREE ? grid_index_sel : grid_index)(hs, g.res[lvl], c[0], c[1], c[2]));
     }
     __half2 r = __floats2half2_rn(0.f, 0.f);
 #pragma unroll

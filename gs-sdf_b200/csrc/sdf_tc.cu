@@ -19,14 +19,15 @@
 // halves). The weight-gradient GEMM dW^T[k][o] = sum_p a[p][k] g[p][o] is an M = 64 wgmma with A = a (MN-major) and B = g (MN-major);
 // four instructions per K step (a_hi, a_mid x g_hi, g_mid) give the 4-term product. Each hidden layer's dW accumulator belongs to one
 // warpgroup and stays in its registers across all tiles of the persistent CTA; it is read out ONCE at the end.
-// Weights are pre-split once per optimiser step (gssdf_sdf_mlp_pack) into that layout (G = 3072: hi | mid | lo) and fetched per
-// layer with one 24 KiB cp.async.bulk (TMA) issued by one thread; completion on an mbarrier.
+// Weights are pre-split once per optimiser step (gssdf_sdf_mlp_pack) into that layout (G = 3072: hi | mid | lo) and fetched with
+// 24 KiB cp.async.bulk (TMA) copies issued by one thread, completion on an mbarrier: per layer in the backward, all layers once per
+// CTA in the forward.
 #include "sdf_grid.cuh"
 #include "sdf_loss.cuh"
 
 namespace gssdf {
 
-constexpr int kFwdTcThreads = 256;   // forward: one 128-point tile per CTA, several CTAs per SM
+constexpr int kFwdTcThreads = 512;   // forward: persistent, one CTA per SM (2 MMA + 2 encode warpgroups)
 constexpr int kBwdTcThreads = 512;   // backward: persistent, one CTA per SM
 constexpr int kLevels = 16;          // check_net: the fused kernels support 16 levels x 2 features
 static_assert(128 * kLevels == 4 * kBwdTcThreads, "encode batches assume 4 tasks per thread");
@@ -231,32 +232,74 @@ __global__ void __launch_bounds__(256) mlp_pack_kernel(const float *__restrict__
 }
 
 // ---------------------------------------------------------------------------------------------
-// forward: persistent CTAs (two per SM) walk the 128-point tiles. The layout stride n is a CAPACITY (the live count is a device value), so
-// most tiles of a launch can be dead: a dead tile costs one loop iteration here instead of a CTA launch, and barrier initialisation
-// and the bias loads happen once per CTA instead of once per tile. Warpgroup wg computes rows 64 wg .. 64 wg + 63 of each tile.
+// forward: persistent, one CTA per SM, warp-specialised. Warpgroups 0-1 (consumers) run the decoder's layers on the tensor cores,
+// warpgroup wg computing rows 64 wg .. 64 wg + 63 of each 128-point tile; warpgroups 2-3 (producers) encode the next tile into the
+// other of two feature buffers meanwhile, so the hash-grid gathers run under the MMAs and epilogues. Every layer's weight image is
+// fetched once per CTA and stays resident. The layout stride n is a CAPACITY (the live count is a device value): tiles are formed from
+// whole points, so the live tiles come first and both roles stop at the same first dead tile; the k-th tile of a CTA always goes
+// through feature buffer k & 1.
+// Hand-offs: full[b] (256 producer arrivals: sF[b] holds the tile's features) and empty[b] (256 consumer arrivals: the layer-0 MMAs
+// are done with sF[b]). The two consumer warpgroups share nothing but the resident weights and each syncs on its own named barrier.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kFwdTcThreads)
+constexpr int kFwdTcConsumers = 256, kFwdTcProducers = 256;
+// (point, level) tasks per producer thread whose 8 gathers each are in flight together. Measured on H100 with uniformly random points
+// (tiles of consecutive evaluation rows): 2 (16 gathers per thread, 4096 per SM) was fastest; 4 was 20 % slower, and 8 gathers per
+// thread 10 % slower.
+constexpr int kFwdEncBatch = 2;
+static_assert((128 * kLevels) % (kFwdEncBatch * kFwdTcProducers) == 0, "encode batches cover the tile");
+constexpr size_t kFwdTcMain = 4 * kWImg + 2 * 16 * kGA0 + 16 * kGA + 16 * kGL;  // resident weights, 2 feature buffers, activations, lo
+constexpr size_t kFwdTcSmem = kFwdTcMain + sizeof(float) * (5 * 64 + 132) + 3 * 2 * sizeof(uint64_t);  // + bias, w_out, mbarriers
+static_assert(kFwdTcSmem + 1024 <= 196 * 1024, "the forward must fit the 196 KiB shared-memory carve-out (L1 keeps 60 KiB for the gathers)");
+
+// barrier `id` over the `n` threads that use it; returns true iff `pred` holds on all of them
+__device__ __forceinline__ bool named_bar_and(int id, int n, bool pred) {
+    uint32_t all;
+    asm volatile(
+        "{\n"
+        ".reg .pred p, q;\n"
+        "setp.ne.b32 p, %1, 0;\n"
+        "bar.red.and.pred q, %2, %3, p;\n"
+        "selp.u32 %0, 1, 0, q;\n"
+        "}\n"
+        : "=r"(all)
+        : "r"((uint32_t)pred), "r"(id), "r"(n)
+        : "memory");
+    return all != 0;
+}
+__device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+__global__ void __launch_bounds__(kFwdTcThreads, 1)
 sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles) {
     constexpr int TM = 128, HID = 64;
     extern __shared__ __align__(128) unsigned char s_tc[];  // (a larger alignment pads the static part and costs the L1 carve-out step)
-    unsigned char *sA = s_tc;                    // 32 KB activations hi/mid (off_act); in place across layers
-    unsigned char *sF = sA + 16 * kGA;           // 16 KB encoded features hi/mid (off_feat)
-    unsigned char *sL = sF + 16 * kGA0;          // 16 KB activation lo (off_lo)
-    unsigned char *sW = sL + 16 * kGL;           // 24 KB weight image of the current layer
-    float *s_bias = reinterpret_cast<float *>(sW + kWImg);  // [5][64]
+    unsigned char *sW = s_tc;                    // 96 KB weight images of all layers (4 x 24 KB), resident
+    unsigned char *sF0 = sW + 4 * kWImg;         // 2 x 16 KB encoded features hi/mid (off_feat), double-buffered
+    unsigned char *sA = sF0 + 2 * 16 * kGA0;     // 32 KB activations hi/mid (off_act); in place across layers
+    unsigned char *sL = sA + 16 * kGA;           // 16 KB activation lo (off_lo)
+    float *s_bias = reinterpret_cast<float *>(sL + 16 * kGL);  // [5][64]
     float *s_wout = s_bias + 5 * 64;             // [2][64] + [2]
-    __shared__ __align__(8) uint64_t s_wbar;     // weight copy
+    uint64_t *s_bar = reinterpret_cast<uint64_t *>(s_wout + 132);  // weights | full[2] | empty[2] (8-byte aligned: 132 floats)
+    uint64_t *s_wbar = s_bar, *s_full = s_bar + 1, *s_empty = s_bar + 3;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int wg = warp >> 2, fr = 64 * wg + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);  // accumulator fragment origin
     const int nh = 1 + a.net.n_hidden;
-    const int64_t n_eval = a.n * max(a.n_variants, 1);
     const int64_t n_live = a.n_live ? min((int64_t)*a.n_live, a.n) : a.n;
-    const __half2 *table = reinterpret_cast<const __half2 *>(a.net.table_half);
-    const unsigned char *wimg = reinterpret_cast<const unsigned char *>(a.net.mlp_packed);
+    // A tile holds PT whole points with their V evaluated variants in consecutive rows (row = j * V + v - v0): the six offsets of a
+    // point lie within a few cells of each other on the coarse levels, so their corner gathers meet in the same load instruction or
+    // in L1 instead of going to L2 six times. skip_base_variant leaves variant 0 out (21 points x 6 + 2 idle rows).
+    const int nv = max(a.n_variants, 1), v0 = (nv == 7 && a.skip_base_variant) ? 1 : 0, V = nv - v0, PT = TM / V;
+    auto eval_of = [&](int64_t tile, int p, bool &live) {  // evaluation index v * n + i of row p (a clamped valid index when idle)
+        const int64_t i = tile * PT + p / V;
+        live = p < PT * V && i < n_live;
+        return (int64_t)(v0 + p % V) * a.n + min(i, a.n - 1);
+    };
 
     if (tid == 0) {
-        mbar_init(&s_wbar, 1);
+        mbar_init(s_wbar, 1);
+        for (int b = 0; b < 2; ++b) {
+            mbar_init(s_full + b, kFwdTcProducers);
+            mbar_init(s_empty + b, kFwdTcConsumers);
+        }
         fence_mbar_init();
     }
     {
@@ -270,82 +313,106 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
     }
     __syncthreads();
     bool ok = true;
-    uint32_t done_layers = 0;  // layers completed by this CTA so far: the weight barrier completes one phase per layer
-    for (int64_t tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
-    const int64_t base = tile * TM;
-    if (base % a.n >= n_live && base % a.n + TM <= a.n) continue;  // CTA-uniform: the whole tile is beyond the live rows
-    if (a.skip_base_variant && base + TM <= a.n) continue;           // CTA-uniform: only variant-0 evaluations in this tile
-    const int tm = (int)min((int64_t)TM, n_eval - base);
-    if (tid == 0) {  // the previous tile's MMAs are complete (every warpgroup waited for them before the last barrier): sW is free
-        mbar_arrive_expect_tx(&s_wbar, kWImg);
-        bulk_g2s(sW, wimg, kWImg, &s_wbar);
-    }
-    // 1. encode: 128 points x 16 levels -> features (global, optional) + A operand of layer 0. Branch-free batches of 4 (point,
-    //    level) tasks per thread so that 32 table gathers are in flight before the first one is consumed.
-    for (int t0 = 0; t0 < TM * kLevels; t0 += 4 * kFwdTcThreads) {
-        float2 f[4];
+    if (warp >= kFwdTcConsumers / 32) {
+        // producers: 1. encode, 128 points x 16 levels -> features (global, optional) + A operand of layer 0. Branch-free batches of
+        // kFwdEncBatch (point, level) tasks per thread (encode_level<true>) so that all their table gathers are in flight before the
+        // first one is consumed.
+        const int ptid = tid - kFwdTcConsumers;
+        const __half2 *table = reinterpret_cast<const __half2 *>(a.net.table_half);
+        uint32_t k = 0;  // live tiles of this CTA so far
+        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+            if (tile * PT >= n_live) break;  // CTA-uniform, the same test in both roles: this and every later tile holds no live point
+            const int b = k & 1;
+            if (k >= 2 && !mbar_wait_bounded(s_empty + b, ((k >> 1) - 1) & 1u)) { ok = false; break; }  // sF[b]'s previous tile is consumed
+            unsigned char *sF = sF0 + b * 16 * kGA0;
+            for (int t0 = 0; t0 < TM * kLevels; t0 += kFwdEncBatch * kFwdTcProducers) {
+                float2 f[kFwdEncBatch];
+                float x[kFwdEncBatch][3];  // load_x first: its 64-bit division branches, which would split the gathers into 8-load groups
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int task = t0 + i * kFwdTcThreads + tid, p = task % TM, lvl = task / TM;
-            float x[3];
-            load_x(a.net, a.x, min(base + p, n_eval - 1), a.n, a.delta, x);
-            f[i] = encode_level(table, g, lvl, x);
-        }
+                for (int i = 0; i < kFwdEncBatch; ++i) {
+                    bool live;
+                    load_x(a.net, a.x, eval_of(tile, (t0 + i * kFwdTcProducers + ptid) % TM, live), a.n, a.delta, x[i]);
+                }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int task = t0 + i * kFwdTcThreads + tid, p = task % TM, lvl = task / TM;
-            const bool live = p < tm && (base + p) % a.n < n_live;
-            if (!live) f[i] = make_float2(0.f, 0.f);
-            if (live && a.feat) *reinterpret_cast<float2 *>(a.feat + (base + p) * kFeat + 2 * lvl) = f[i];
-            __nv_bfloat16 h0, m0, h1, m1;
-            split2(f[i].x, h0, m0);
-            split2(f[i].y, h1, m1);
-            *reinterpret_cast<__nv_bfloat162 *>(sF + off_feat(p, 2 * lvl, 0)) = __halves2bfloat162(h0, h1);
-            *reinterpret_cast<__nv_bfloat162 *>(sF + off_feat(p, 2 * lvl, 1)) = __halves2bfloat162(m0, m1);
-        }
-    }
-    for (int l = 0; l < nh; ++l) {
-        fence_proxy_async();  // generic-proxy writes of the A operand -> visible to the tensor core
-        ok = __syncthreads_and(mbar_wait_bounded(&s_wbar, (done_layers + (uint32_t)l) & 1u));  // W_l has landed
-        if (!ok) break;
-        float d[32];
-        issue_forward_layer(d, l, smem_u32(l == 0 ? sF + 8 * wg * kGA0 : sA + 8 * wg * kGA), smem_u32(sL + 8 * wg * kGL), smem_u32(sW));
-        wg_wait();
-        acc_fence(d);
-        __syncthreads();  // every warpgroup's MMAs are done with sW: fetch the next layer while the epilogue runs
-        if (tid == 0 && l + 1 < nh) {
-            mbar_arrive_expect_tx(&s_wbar, kWImg);
-            bulk_g2s(sW, wimg + (size_t)(l + 1) * kWImg, kWImg, &s_wbar);
-        }
-        float act[32];
+                for (int i = 0; i < kFwdEncBatch; ++i) f[i] = encode_level<true>(table, g, (t0 + i * kFwdTcProducers + ptid) / TM, x[i]);
 #pragma unroll
-        for (int e = 0; e < 32; ++e) act[e] = fmaxf(d[e] + s_bias[l * 64 + 8 * (e >> 2) + fc + (e & 1)], 0.f);
-        if (l < nh - 1) {  // rows of this warpgroup only: sA is rewritten in place
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) store2(sA, sL, fr + 8 * ((e >> 1) & 1), 8 * (e >> 2) + fc, act[e], act[e + 1]);
-        } else {  // output layer (64 -> 2) on the CUDA cores, straight from the registers; a quad holds a whole row
-            float p0[2] = {0.f, 0.f}, p1[2] = {0.f, 0.f};
-#pragma unroll
-            for (int e = 0; e < 32; ++e) {
-                const int i = (e >> 1) & 1, c = 8 * (e >> 2) + fc + (e & 1);
-                p0[i] = fmaf(act[e], s_wout[c], p0[i]);
-                p1[i] = fmaf(act[e], s_wout[HID + c], p1[i]);
-            }
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const float s0 = quad_sum(p0[i]), s1 = quad_sum(p1[i]);
-                const int p = fr + 8 * i;
-                if ((lane & 3) == 0 && p < tm && (base + p) % a.n < n_live) {
-                    a.sdf[base + p] = s0 + s_wout[2 * HID];
-                    if (a.y1) a.y1[base + p] = s1 + s_wout[2 * HID + 1];
+                for (int i = 0; i < kFwdEncBatch; ++i) {
+                    const int task = t0 + i * kFwdTcProducers + ptid, p = task % TM, lvl = task / TM;
+                    bool live;
+                    const int64_t e = eval_of(tile, p, live);
+                    if (!live) f[i] = make_float2(0.f, 0.f);
+                    if (live && a.feat) *reinterpret_cast<float2 *>(a.feat + e * kFeat + 2 * lvl) = f[i];
+                    __nv_bfloat16 h0, m0, h1, m1;
+                    split2(f[i].x, h0, m0);
+                    split2(f[i].y, h1, m1);
+                    *reinterpret_cast<__nv_bfloat162 *>(sF + off_feat(p, 2 * lvl, 0)) = __halves2bfloat162(h0, h1);
+                    *reinterpret_cast<__nv_bfloat162 *>(sF + off_feat(p, 2 * lvl, 1)) = __halves2bfloat162(m0, m1);
                 }
             }
+            fence_proxy_async();  // generic-proxy writes of the A operand -> visible to the tensor core
+            mbar_arrive(s_full + b);
+            ++k;
+        }
+    } else {
+        // consumers: the decoder's layers on this warpgroup's 64 rows
+        const int wg = warp >> 2, fr = 64 * wg + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);  // accumulator fragment origin
+        const int bar_id = 1 + wg;
+        const unsigned char *wimg = reinterpret_cast<const unsigned char *>(a.net.mlp_packed);
+        uint32_t k = 0;
+        for (int64_t tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
+            if (tile * PT >= n_live) break;  // CTA-uniform, the same test in both roles: this and every later tile holds no live point
+            const int b = k & 1;
+            bool landed = true;
+            if (k == 0) {  // the first live tile of this CTA fetches every layer's weights (a CTA without one never starts a copy)
+                if (tid == 0) {
+                    mbar_arrive_expect_tx(s_wbar, (uint32_t)nh * kWImg);
+                    for (int l = 0; l < nh; ++l) bulk_g2s(sW + l * kWImg, wimg + (size_t)l * kWImg, kWImg, s_wbar);
+                }
+                landed = mbar_wait_bounded(s_wbar, 0);
+            }
+            for (int l = 0; l < nh; ++l) {
+                if (l == 0) landed = landed && mbar_wait_bounded(s_full + b, (k >> 1) & 1u);  // the tile's features have landed
+                else fence_proxy_async();  // generic-proxy writes of the A operand -> visible to the tensor core
+                ok = named_bar_and(bar_id, 128, landed);
+                if (!ok) break;
+                float d[32];
+                issue_forward_layer(d, l, smem_u32(l == 0 ? sF0 + b * 16 * kGA0 + 8 * wg * kGA0 : sA + 8 * wg * kGA), smem_u32(sL + 8 * wg * kGL),
+                                    smem_u32(sW + l * kWImg));
+                wg_wait();
+                acc_fence(d);
+                if (l == 0) mbar_arrive(s_empty + b);  // sF[b] is free for the tile after next
+                else if (l < nh - 1) named_bar(bar_id, 128);  // the warpgroup's MMAs are done with sA / sL: the epilogue rewrites them
+                float act[32];
+#pragma unroll
+                for (int e = 0; e < 32; ++e) act[e] = fmaxf(d[e] + s_bias[l * 64 + 8 * (e >> 2) + fc + (e & 1)], 0.f);
+                if (l < nh - 1) {  // rows of this warpgroup only: sA is rewritten in place
+#pragma unroll
+                    for (int e = 0; e < 32; e += 2) store2(sA, sL, fr + 8 * ((e >> 1) & 1), 8 * (e >> 2) + fc, act[e], act[e + 1]);
+                } else {  // output layer (64 -> 2) on the CUDA cores, straight from the registers; a quad holds a whole row
+                    float p0[2] = {0.f, 0.f}, p1[2] = {0.f, 0.f};
+#pragma unroll
+                    for (int e = 0; e < 32; ++e) {
+                        const int i = (e >> 1) & 1, c = 8 * (e >> 2) + fc + (e & 1);
+                        p0[i] = fmaf(act[e], s_wout[c], p0[i]);
+                        p1[i] = fmaf(act[e], s_wout[HID + c], p1[i]);
+                    }
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const float s0 = quad_sum(p0[i]), s1 = quad_sum(p1[i]);
+                        const int p = fr + 8 * i;
+                        bool live;
+                        const int64_t e = eval_of(tile, p, live);
+                        if ((lane & 3) == 0 && live) {
+                            a.sdf[e] = s0 + s_wout[2 * HID];
+                            if (a.y1) a.y1[e] = s1 + s_wout[2 * HID + 1];
+                        }
+                    }
+                }
+            }
+            ++k;
         }
     }
-    done_layers += (uint32_t)nh;
-    __syncthreads();  // sF / sA are rewritten by the next tile
-    }  // tile loop
-    if (!ok) __trap();  // the copy engine never signalled: fail loudly rather than return garbage
+    if (!ok) __trap();  // a copy or a hand-off never completed: fail loudly rather than return garbage
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -967,18 +1034,18 @@ static int check_tc(const char *who, const gssdf_sdf_net &net) {
 extern "C" int gssdf_sdf_fwd_tc_launch(const gssdf_sdf_fwd_args *a, const gssdf::GridGeom *g, gssdf_stream_t stream) {
     int rc = check_tc("sdf_fwd", a->net);
     if (rc) return rc;
-    const size_t smem = 16 * kGA + 16 * kGA0 + 16 * kGL + kWImg + sizeof(float) * (5 * 64 + 132) + 1024;
     static bool attr_set = false;
     if (!attr_set) {
-        GSSDF_CUDA_OK(cudaFuncSetAttribute(sdf_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        GSSDF_CUDA_OK(cudaFuncSetAttribute(sdf_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFwdTcSmem));
         attr_set = true;
     }
-    const int64_t n_tiles = (a->n * (a->n_variants > 1 ? a->n_variants : 1) + 127) / 128;
+    const int nv = a->n_variants > 1 ? a->n_variants : 1, pt = 128 / (nv == 7 && a->skip_base_variant ? 6 : nv);  // points per tile
+    const int64_t n_tiles = (a->n + pt - 1) / pt;
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)2 * sms);  // two ~90 KiB CTAs fit one SM
-    sdf_fwd_tc_kernel<<<grid, kFwdTcThreads, smem, (cudaStream_t)stream>>>(*a, *g, n_tiles);
+    const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms);
+    sdf_fwd_tc_kernel<<<grid, kFwdTcThreads, kFwdTcSmem, (cudaStream_t)stream>>>(*a, *g, n_tiles);
     GSSDF_LAUNCH_OK("sdf_fwd_tc_kernel");
     return GSSDF_OK;
 }

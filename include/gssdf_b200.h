@@ -456,7 +456,8 @@ typedef struct gssdf_sdf_fwd_args {
     float *sdf;       /* [n_variants*n] decoder output 0 */
     float *y1;        /* [n_variants*n] decoder output 1 (raw; isigma = 1 + softplus_100(y1) * k_bce_isigma) or NULL */
     float *feat;      /* [n_variants*n, L*F] encoding (fp16-exact values) or NULL */
-    int32_t skip_base_variant; /* 1 (n_variants 7): tiles that hold only variant-0 evaluations are skipped (their outputs stay untouched):
+    int32_t skip_base_variant; /* 1 (n_variants 7): variant 0 need not be evaluated (mlp_mode 1: none of its outputs is written;
+                                  mlp_mode 0: tiles that hold only variant-0 evaluations are skipped, their outputs stay untouched):
                                   the caller needs the six offsets only (numerical gradient next to gssdf_sdf_train on the base points) */
 } gssdf_sdf_fwd_args;
 int gssdf_sdf_fwd(const gssdf_sdf_fwd_args *a, gssdf_stream_t stream);
