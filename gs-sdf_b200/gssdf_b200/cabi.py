@@ -3,6 +3,8 @@
 One function per entry point of include/gssdf_b200.h. Nothing here computes: every function fills an
 args struct with raw device pointers and calls libgssdf_b200.so on torch's current CUDA stream.
 """
+import math
+
 import torch
 
 from . import _lib
@@ -373,6 +375,23 @@ def sdf_gate_compact(n, x, index, x_out, n_gate, ws, visibilities=None, visible_
     a = make_args("gssdf_sdf_gate_compact_args", n=n, n_live=n_live, visibilities=visibilities, visible_thr=visible_thr, valid_mask=valid_mask,
                   x=x, weights=weights, index=index, x_out=x_out, w_out=w_out, n_gate=n_gate, workspace=w, workspace_bytes=w.numel())
     check(lib().gssdf_sdf_gate_compact(_lib.C.byref(a), _stream()))
+
+
+def sdf_outlier_filter(net, xyz, threshold, columns, n_kept, ws, index=None, n=None):
+    """Rows r < n (default: all of xyz) with |sdf(xyz[r])| < threshold (fp32), in order: index[j] = j-th kept row (or None), *n_kept = count
+    (device int64 [1]), and for each (src, dst) of `columns` (contiguous CUDA tensors of equal row width) dst[j] = src[index[j]]."""
+    n = xyz.shape[0] if n is None else int(n)
+    w = ws.get(lib().gssdf_sdf_outlier_filter_workspace_bytes(_lib.C.c_int64(n)))
+    a = make_args("gssdf_sdf_outlier_filter_args", n=n, xyz=_req(xyz, torch.float32, "xyz"), threshold=threshold, n_columns=len(columns),
+                  index=_req(index, torch.int64, "index"), n_kept=_req(n_kept, torch.int64, "n_kept"), workspace=w, workspace_bytes=w.numel())
+    a.net = net
+    for i, (src, dst) in enumerate(columns[:len(a.columns)]):  # more columns than the struct holds: n_columns makes the library refuse
+        for name, t in (("src", src), ("dst", dst)):
+            if not (t.is_cuda and t.is_contiguous()):
+                raise ValueError(f"gssdf_b200: column {i} {name} must be a contiguous CUDA tensor")
+        a.columns[i].src, a.columns[i].dst = src.data_ptr() or None, dst.data_ptr() or None
+        a.columns[i].row_bytes = math.prod(src.shape[1:]) * src.element_size()
+    check(lib().gssdf_sdf_outlier_filter(_lib.C.byref(a), _stream()))
 
 
 def scatter_rows3(n, index, n_gate, src, dst, n_live=None):

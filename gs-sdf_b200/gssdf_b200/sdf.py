@@ -5,11 +5,15 @@ Reference (paths relative to /root/reference):
                                           submodules/tcnn_binding/tcnn_binding/tcnn_binding.h:16-105
   LocalMap::get_sdf(xyz) -> {sdf, isigma}  include/neural_net/local_map.cpp:87-103
   LocalMap::get_gradient(xyz, delta, ..., numerical) include/neural_net/local_map.cpp:105-173 (numerical branch)
+  NeuralSLAM::sdf_train_callback's outlier branch  include/neural_mapping/neural_mapping.cpp:559-592 (remove_outliers)
 `params_` stays a flat fp32 [n_params] torch parameter (checkpoint layout of torch::save(local_map_ptr)).
 All compute is in libgssdf_b200.so; autograd is plumbing.
 """
+import ctypes
+import ctypes.util
 import math
 
+import numpy as np
 import torch
 
 from . import cabi
@@ -100,3 +104,71 @@ class SdfNet(torch.nn.Module):
         pts = (xyz.unsqueeze(0) + offs).view(-1, 3)
         s = self.get_sdf(pts)[0].view(6, xyz.shape[0], 1)
         return 0.5 / delta * torch.cat([s[0] - s[1], s[2] - s[3], s[4] - s[5]], 1)
+
+
+_libm = None
+
+
+def _m():
+    """The host's libm: the threshold is computed with the same logf / log / exp the reference's C++ calls."""
+    global _libm
+    if _libm is None:
+        L = ctypes.CDLL(ctypes.util.find_library("m") or "libm.so.6")
+        L.logf.restype, L.logf.argtypes = ctypes.c_float, [ctypes.c_float]
+        for fn in (L.log, L.exp):
+            fn.restype, fn.argtypes = ctypes.c_double, [ctypes.c_double]
+        _libm = L
+    return _libm
+
+
+def outlier_threshold(it, total_it, truncated_dis, outlier_dist):
+    """The fp32 threshold of sdf_train_callback's outlier removal (neural_mapping.cpp:542,565-566), one rounding at a time:
+    iter_ratio = (float)it / total_it in fp32; exp(logf(truncated_dis) * (1 - iter_ratio) + log(outlier_dist) * iter_ratio) with the first
+    product in fp32 (k_truncated_dis is a float) and the rest in double; then rounded once to fp32, which is what `tensor < double` compares
+    against."""
+    f, m = np.float32, _m()
+    ratio = f(it) / f(total_it)
+    a = f(m.logf(float(f(truncated_dis)))) * (f(1) - ratio)
+    return float(f(m.exp(float(a) + m.log(float(outlier_dist)) * float(ratio))))
+
+
+def outlier_rows(N, vis_batch_pt_num=1_638_400):
+    """How many leading rows of an N-row pack the reference's chunk loop can keep. It evaluates rows [i, min(i + B, N - 1)) for
+    i = 0, B, 2B, ..., so never the last row. A chunk of exactly one row (B == 1, or the last chunk when (N - 1) % B == 1) keeps nothing:
+    `.squeeze()` makes its mask 0-d, and nonzero() of a 0-d True squeezes to an empty index (of a 0-d False to a [0,0] one, which makes
+    the reference throw)."""
+    n, b = max(N - 1, 0), vis_batch_pt_num
+    if b == 1:
+        return 0
+    return n - 1 if n % b == 1 else n
+
+
+def remove_outliers(net, pack, it, total_it, *, truncated_dis, outlier_dist, interval, vis_batch_pt_num=1_638_400, ws=None):
+    """sdf_train_callback's outlier branch (neural_mapping.cpp:559-592) on a depth pack: a dict of [N, k] tensors with the points under
+    "xyz" (e.g. origin, direction, depth, xyz). At it > 0 with it % interval == 0, keeps the rows r < outlier_rows(N, vis_batch_pt_num)
+    with |net.get_sdf(xyz[r])| < outlier_threshold(...) in every field, in order: the last row is never evaluated, as in the reference.
+    Other iterations return the pack unchanged. Returns (pack, number of rows); the count is read back once.
+    A CUDA pack is compacted on the device by gssdf_sdf_outlier_filter (the fields are views of the first rows of new N-row buffers). A CPU
+    pack (where the reference keeps it) sends xyz to the device once and index_selects every field on the host with the kept rows.
+    Where the reference throws (N == 0, a chunk with exactly one kept row among several), the pack is empty, or the row kept."""
+    N = pack["xyz"].shape[0]
+    if not (it > 0 and it % interval == 0):
+        return pack, N
+    thr = outlier_threshold(it, total_it, truncated_dis, outlier_dist)
+    n = outlier_rows(N, vis_batch_pt_num)
+    dev = net.params_.device
+    ws = cabi.Workspace(dev) if ws is None else ws
+    n_kept = torch.empty(1, dtype=torch.int64, device=dev)
+    ns = net._net(net.params_, net.decoder_)
+    xyz = pack["xyz"].reshape(N, 3)
+    if xyz.is_cuda:
+        out = {k: torch.empty_like(v, memory_format=torch.contiguous_format) for k, v in pack.items()}
+        cols = [(v.contiguous(), out[k]) for k, v in pack.items()]
+        cabi.sdf_outlier_filter(ns, xyz.contiguous(), thr, cols, n_kept, ws, n=n)
+        kept = int(n_kept.item())
+        return {k: v[:kept] for k, v in out.items()}, kept
+    index = torch.empty(n, dtype=torch.int64, device=dev)
+    cabi.sdf_outlier_filter(ns, xyz[:n].to(dev, torch.float32).contiguous(), thr, [], n_kept, ws, index=index, n=n)
+    kept = int(n_kept.item())
+    idx = index[:kept].cpu()
+    return {k: v.index_select(0, idx) for k, v in pack.items()}, kept

@@ -1,5 +1,6 @@
 // Python binding of the libtorch shim (test harness only): lets the GPU tests drive the SAME C++ entry points that
 // neural_gaussian.cpp would call (gs-sdf_b200/shim/include/gsplat_cpp/*.h), end to end through autograd.
+#include <ATen/cuda/CUDAContext.h>
 #include <torch/extension.h>
 
 #include "gsplat_cpp/fully_fused_projection.h"
@@ -10,6 +11,7 @@
 #include "gssdf_mesh.hpp"
 #include "gssdf_metrics.hpp"
 #include "gssdf_octree.hpp"
+#include "gssdf_sdf_net.hpp"
 #include "spatial.h"
 
 void bind_tcnn(pybind11::module &m);
@@ -51,6 +53,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                        const torch::Tensor &xyzs, float mesh_res, bool init_opa) {
         torch::nn::Sequential decoder = make_decoder((int64_t)encoder->get_out_dim(), decoder_flat, hidden_dim, geo_num_layer);
         return gssdf::init_gs_with_sdf(*encoder, decoder, pos_W_M, map_size, bce_isigma, xyzs, mesh_res, init_opa);
+    });
+    m.def("gssdf_remove_outliers", [](const std::shared_ptr<TCNNEncoding> &encoder, const torch::Tensor &decoder_flat, int hidden_dim,
+                                      int geo_num_layer, const torch::Tensor &pos_W_M, float map_size, const torch::Tensor &xyz,
+                                      const std::vector<torch::Tensor> &fields, int iter, int total_iter, float truncated_dis,
+                                      double outlier_dist, int vis_batch_pt_num) {
+        torch::nn::Sequential decoder = make_decoder((int64_t)encoder->get_out_dim(), decoder_flat, hidden_dim, geo_num_layer);
+        auto stream = reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream());
+        const gssdf::SdfNetHolder holder = gssdf::make_sdf_net(*encoder, decoder, pos_W_M, map_size, stream);
+        return gssdf::remove_outliers(holder, xyz, fields, iter, total_iter, truncated_dis, outlier_dist, vis_batch_pt_num);
     });
     m.def("gssdf_cull_mesh_accumulate", [](torch::Tensor seen, const torch::Tensor &vertices, const torch::Tensor &depths,
                                            const torch::Tensor &c2w, float fx, float fy, float cx, float cy, int W, int H) {

@@ -1276,6 +1276,43 @@ typedef struct gssdf_image_metrics_args {
 size_t gssdf_image_metrics_workspace_bytes(int32_t V, int32_t W, int32_t H);
 int gssdf_image_metrics(const gssdf_image_metrics_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-12  Outlier removal of the training depth pack.  Replaces the outlier branch of NeuralSLAM::sdf_train_callback
+ *     (include/neural_mapping/neural_mapping.cpp:559-592): evaluate the SDF on every row of the pack and keep the rows with |sdf| < thr,
+ *     in order, in every field of the pack (DESIGN 7m). One call, no allocation, no sync; all arguments are checked before the first
+ *     launch; bit-identical from run to run and capturable in a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+/* sdf_r = gssdf_sdf_fwd(net, xyz[r]) (n_variants 1, decoder output 0, any mlp_mode), r < n. Row r is kept when fabsf(sdf_r) < threshold
+   in fp32 (a NaN SDF is dropped). index[j] = the j-th kept row, ascending (nonzero()'s order); *n_kept = their number; for every column,
+   row j of dst = row index[j] of src, rows [*n_kept, n) of dst and index untouched. The reference never evaluates its last row
+   (`end = min(i + B, N - 1)`) and keeps nothing from a chunk of one row: pass n = N - 1, or N - 2 when (N - 1) % B == 1
+   (gssdf_b200.sdf.outlier_rows), to reproduce its pack. Unlike the reference, a chunk with exactly one kept row and N == 0 are not
+   errors (DESIGN 7m).
+   GSSDF_EINVAL before any launch for n < 0, n_columns outside [0, GSSDF_OUTLIER_MAX_COLUMNS], a NULL n_kept, when n > 0 a NULL xyz,
+   src, dst or workspace, a row_bytes that is not a positive multiple of 4 (at most 2^20), a dst that overlaps any column's src or
+   another column's dst, or a workspace that is too small; gssdf_sdf_fwd's own checks of net apply too (also for n == 0). */
+#define GSSDF_OUTLIER_MAX_COLUMNS 8
+typedef struct gssdf_column {
+    const void *src;              /* [n] rows of row_bytes */
+    void *dst;                    /* [n] rows of row_bytes, rows [0, *n_kept) written */
+    int64_t row_bytes;
+} gssdf_column;
+typedef struct gssdf_sdf_outlier_filter_args {
+    gssdf_sdf_net net;
+    int64_t n;                    /* rows evaluated */
+    const float *xyz;             /* [n,3] */
+    float threshold;
+    int32_t n_columns;
+    gssdf_column columns[GSSDF_OUTLIER_MAX_COLUMNS];
+    int64_t *index;               /* [n] or NULL */
+    int64_t *n_kept;              /* device int64, overwritten */
+    void *workspace;              /* >= gssdf_sdf_outlier_filter_workspace_bytes(n) */
+    size_t workspace_bytes;
+} gssdf_sdf_outlier_filter_args;
+/* 0 for n < 0 */
+size_t gssdf_sdf_outlier_filter_workspace_bytes(int64_t n);
+int gssdf_sdf_outlier_filter(const gssdf_sdf_outlier_filter_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
