@@ -198,10 +198,12 @@ struct __align__(16) StagedHit {
     int32_t pad;
 };
 
-__global__ void __launch_bounds__(kRayThreads) ray_count_kernel(const gssdf_octree t, int n_cached, int64_t n, const float *origins, const float *dirs,
-                                                                int32_t *cnt, StagedHit *stage) {
+// n_live (device int32 or NULL): rays >= *n_live are not traced (a capacity-sized batch with a device ray count)
+__global__ void __launch_bounds__(kRayThreads) ray_count_kernel(const gssdf_octree t, int n_cached, int64_t n, const int32_t *n_live,
+                                                                const float *origins, const float *dirs, int32_t *cnt, StagedHit *stage) {
     extern __shared__ __align__(16) unsigned char s_tree[];
     __shared__ RayStack s_stack;
+    if (n_live) n = min(n, (int64_t)*n_live);
     const TreeView tv = stage_tree(t, n_cached, s_tree);
     const int64_t i = (int64_t)blockIdx.x * kRaysPerCta + threadIdx.x / kRayLanes;
     if (i >= n) return;  // (all eight lanes of a ray leave together)
@@ -213,11 +215,12 @@ __global__ void __launch_bounds__(kRayThreads) ray_count_kernel(const gssdf_octr
     if (threadIdx.x % kRayLanes == 0) cnt[i] = k;
 }
 
-__global__ void __launch_bounds__(kRayThreads) ray_write_kernel(const gssdf_octree t, int n_cached, int64_t n, const float *origins, const float *dirs,
-                                                                const int32_t *cnt, const int32_t *off, const StagedHit *stage, int64_t cap,
-                                                                int32_t *ridx, int32_t *pidx, float *depth) {
+__global__ void __launch_bounds__(kRayThreads) ray_write_kernel(const gssdf_octree t, int n_cached, int64_t n, const int32_t *n_live,
+                                                                const float *origins, const float *dirs, const int32_t *cnt, const int32_t *off,
+                                                                const StagedHit *stage, int64_t cap, int32_t *ridx, int32_t *pidx, float *depth) {
     extern __shared__ __align__(16) unsigned char s_tree[];
     __shared__ RayStack s_stack;
+    if (n_live) n = min(n, (int64_t)*n_live);
     const int64_t i = (int64_t)blockIdx.x * kRaysPerCta + threadIdx.x / kRayLanes;
     const int g = threadIdx.x % kRayLanes;
     const int k = i < n ? cnt[i] : 0;
@@ -387,9 +390,11 @@ __device__ __forceinline__ float f_scale_from_m1p1(const gssdf_octree &t, float 
 }
 
 // candidate c of the reference's concatenation [voxel samples | free samples | surface samples | ray end points]
-__device__ __forceinline__ Cand make_candidate(const gssdf_sdf_sample_rays_args &a, int64_t c, int64_t n_vox, const int32_t *nug_ridx, const float *nug_depth) {
+// n = live rays (a.n_rays, or fewer with gssdf_sdf_sample_rays_dev), std = the surface samples' std (a.sample_std or the device value)
+__device__ __forceinline__ Cand make_candidate(const gssdf_sdf_sample_rays_args &a, int64_t n, float std, int64_t c, int64_t n_vox, const int32_t *nug_ridx,
+                                               const float *nug_depth) {
     Cand s;
-    const int64_t n = a.n_rays, n_free = (int64_t)a.n_free * n, n_surf = (int64_t)a.n_surface * n;
+    const int64_t n_free = (int64_t)a.n_free * n, n_surf = (int64_t)a.n_surface * n;
     int seg;
     int64_t q = c;
     if (q < n_vox) seg = 0;
@@ -435,7 +440,7 @@ __device__ __forceinline__ Cand make_candidate(const gssdf_sdf_sample_rays_args 
         s.keep = rs > 0.f;
     } else if (seg == 2) {  // utils::sample_surface_pts
         r = q / a.n_surface;
-        rs = __fmul_rn(__ldg(a.randn_surface + q), a.sample_std);
+        rs = __fmul_rn(__ldg(a.randn_surface + q), std);
         dep = __ldg(a.depth + r);
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
@@ -461,23 +466,30 @@ __device__ __forceinline__ Cand make_candidate(const gssdf_sdf_sample_rays_args 
     return s;
 }
 
-__global__ void __launch_bounds__(256) sample_flag_kernel(const gssdf_sdf_sample_rays_args a, const int32_t *nug_ridx, const float *nug_depth, int32_t *flags,
-                                                          int64_t m_cap) {
-    const int64_t c = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    const int64_t n_vox = (int64_t)min((int64_t)a.counts[1], a.nugget_cap) * a.voxel_sample_num;
-    const int64_t m = n_vox + (int64_t)a.n_rays * (a.n_free + a.n_surface + 1);
-    if (c >= m_cap) return;
-    flags[c] = c < m ? (make_candidate(a, c, n_vox, nug_ridx, nug_depth).keep ? 1 : 0) : 0;
+// n_live / std_dev: device overrides of a.n_rays (a bound) and a.sample_std, or NULL
+__device__ __forceinline__ int64_t live_rays(const gssdf_sdf_sample_rays_args &a, const int32_t *n_live) {
+    return n_live ? min(a.n_rays, (int64_t)*n_live) : a.n_rays;
 }
 
-__global__ void __launch_bounds__(256) sample_write_kernel(const gssdf_sdf_sample_rays_args a, const int32_t *nug_ridx, const float *nug_depth,
-                                                           const int32_t *flags, const int32_t *pos, int64_t m_cap) {
+__global__ void __launch_bounds__(256) sample_flag_kernel(const gssdf_sdf_sample_rays_args a, const int32_t *n_live, const float *std_dev,
+                                                          const int32_t *nug_ridx, const float *nug_depth, int32_t *flags, int64_t m_cap) {
+    const int64_t c = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    const int64_t n = live_rays(a, n_live);
+    const int64_t n_vox = (int64_t)min((int64_t)a.counts[1], a.nugget_cap) * a.voxel_sample_num;
+    const int64_t m = n_vox + n * (a.n_free + a.n_surface + 1);
+    if (c >= m_cap) return;
+    flags[c] = c < m ? (make_candidate(a, n, std_dev ? *std_dev : a.sample_std, c, n_vox, nug_ridx, nug_depth).keep ? 1 : 0) : 0;
+}
+
+__global__ void __launch_bounds__(256) sample_write_kernel(const gssdf_sdf_sample_rays_args a, const int32_t *n_live, const float *std_dev,
+                                                           const int32_t *nug_ridx, const float *nug_depth, const int32_t *flags, const int32_t *pos,
+                                                           int64_t m_cap) {
     const int64_t c = (int64_t)blockIdx.x * 256 + threadIdx.x;
     if (c >= m_cap || !flags[c]) return;
     const int64_t n_vox = (int64_t)min((int64_t)a.counts[1], a.nugget_cap) * a.voxel_sample_num;
     const int64_t p = pos[c];
     if (p >= a.cap) return;
-    const Cand s = make_candidate(a, c, n_vox, nug_ridx, nug_depth);
+    const Cand s = make_candidate(a, live_rays(a, n_live), std_dev ? *std_dev : a.sample_std, c, n_vox, nug_ridx, nug_depth);
     a.out_xyz[3 * p] = s.xyz[0]; a.out_xyz[3 * p + 1] = s.xyz[1]; a.out_xyz[3 * p + 2] = s.xyz[2];
     a.out_ray_sdf[p] = s.ray_sdf;
     if (a.out_direction) { a.out_direction[3 * p] = s.dir[0]; a.out_direction[3 * p + 1] = s.dir[1]; a.out_direction[3 * p + 2] = s.dir[2]; }
@@ -631,20 +643,21 @@ extern "C" size_t gssdf_octree_raytrace_workspace_bytes(int64_t n_rays) {
     return L.bytes();
 }
 
-static int raytrace_impl(const gssdf_octree &tree, int64_t n_rays, const float *origins, const float *dirs, int64_t cap, int32_t *ridx, int32_t *pidx,
-                         float *depth, int32_t *n_nuggets, int32_t *overflow, const RayWs &w, cudaStream_t st) {
+// n_live: device int32 or NULL, rays >= *n_live are not traced (n_rays stays the capacity of the batch and of the workspace)
+static int raytrace_impl(const gssdf_octree &tree, int64_t n_rays, const int32_t *n_live, const float *origins, const float *dirs, int64_t cap,
+                         int32_t *ridx, int32_t *pidx, float *depth, int32_t *n_nuggets, int32_t *overflow, const RayWs &w, cudaStream_t st) {
     GSSDF_CUDA_OK(cudaMemsetAsync(n_nuggets, 0, sizeof(int32_t), st));
     if (n_rays == 0 || tree.n_nodes == 0) return GSSDF_OK;
     const int n_cached = std::min(tree.n_nodes, kTreeCacheNodes);
     const size_t smem = (size_t)n_cached * 5 + 16;
     GSSDF_CUDA_OK(cudaFuncSetAttribute(ray_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTreeCacheNodes * 5 + 16));
     GSSDF_CUDA_OK(cudaFuncSetAttribute(ray_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTreeCacheNodes * 5 + 16));
-    ray_count_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, origins, dirs, w.cnt, w.stage);
+    ray_count_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, n_live, origins, dirs, w.cnt, w.stage);
     GSSDF_LAUNCH_OK("ray_count_kernel");
-    scan_kernel<<<1, 1024, 0, st>>>(w.cnt, w.off, n_rays, nullptr, cap, n_nuggets, overflow);
+    scan_kernel<<<1, 1024, 0, st>>>(w.cnt, w.off, n_rays, n_live, cap, n_nuggets, overflow);
     GSSDF_LAUNCH_OK("scan_kernel");
-    ray_write_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, origins, dirs, w.cnt, w.off, w.stage, cap, ridx,
-                                                                          pidx, depth);
+    ray_write_kernel<<<cdiv(n_rays, kRaysPerCta), kRayThreads, smem, st>>>(tree, n_cached, n_rays, n_live, origins, dirs, w.cnt, w.off, w.stage, cap,
+                                                                          ridx, pidx, depth);
     GSSDF_LAUNCH_OK("ray_write_kernel");
     return GSSDF_OK;
 }
@@ -660,7 +673,7 @@ extern "C" int gssdf_octree_raytrace(const gssdf_octree_raytrace_args *a, gssdf_
     const RayWs w = take_ray_ws(L, a->n_rays);
     GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= L.bytes(), GSSDF_ENOMEM, "octree_raytrace: workspace too small");
     GSSDF_CUDA_OK(cudaMemsetAsync(a->n_nuggets, 0, 2 * sizeof(int32_t), (cudaStream_t)stream));
-    return raytrace_impl(a->tree, a->n_rays, a->origins, a->dirs, a->cap, a->ridx, a->pidx, a->depth, a->n_nuggets, a->n_nuggets + 1, w,
+    return raytrace_impl(a->tree, a->n_rays, nullptr, a->origins, a->dirs, a->cap, a->ridx, a->pidx, a->depth, a->n_nuggets, a->n_nuggets + 1, w,
                          (cudaStream_t)stream);
 }
 
@@ -693,7 +706,8 @@ extern "C" size_t gssdf_sdf_sample_rays_workspace_bytes(int64_t n_rays, int64_t 
     return sample_rays_ws(n_rays, nugget_cap, sample_cand_cap(n_rays, nugget_cap, ns, n_free, n_surface), nullptr).bytes;
 }
 
-extern "C" int gssdf_sdf_sample_rays(const gssdf_sdf_sample_rays_args *a, gssdf_stream_t stream) {
+// n_live / std_dev: gssdf_sdf_sample_rays_dev's device ray count and std (NULL: a->n_rays / a->sample_std)
+static int sample_rays_impl(const gssdf_sdf_sample_rays_args *a, const int32_t *n_live, const float *std_dev, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "sdf_sample_rays: null args");
     GSSDF_REQUIRE(a->n_rays >= 0 && a->cap >= 0 && a->nugget_cap >= 0, GSSDF_EINVAL, "sdf_sample_rays: negative size");
     GSSDF_REQUIRE(a->voxel_sample_num >= 1 && a->n_free >= 0 && a->n_surface >= 0, GSSDF_EINVAL, "sdf_sample_rays: bad sample counts");
@@ -711,16 +725,23 @@ extern "C" int gssdf_sdf_sample_rays(const gssdf_sdf_sample_rays_args *a, gssdf_
     GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "sdf_sample_rays: workspace too small (%zu < %zu)", a->workspace_bytes,
                   w.bytes);
     GSSDF_REQUIRE(m_cap < ((int64_t)1 << 31), GSSDF_EINVAL, "sdf_sample_rays: too many candidates for one call");
-    rc = raytrace_impl(a->tree, a->n_rays, a->origin, a->direction, a->nugget_cap, w.nug_ridx, nullptr, w.nug_depth, a->counts + 1, a->counts + 2,
-                       w.ray, st);
+    rc = raytrace_impl(a->tree, a->n_rays, n_live, a->origin, a->direction, a->nugget_cap, w.nug_ridx, nullptr, w.nug_depth, a->counts + 1,
+                       a->counts + 2, w.ray, st);
     if (rc) return rc;
-    sample_flag_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, w.nug_ridx, w.nug_depth, w.flags, m_cap);
+    sample_flag_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, n_live, std_dev, w.nug_ridx, w.nug_depth, w.flags, m_cap);
     GSSDF_LAUNCH_OK("sample_flag_kernel");
     rc = run_scan(w.flags, w.pos, m_cap, nullptr, a->cap, a->counts, a->counts + 2, w.scan_scratch, st);
     if (rc) return rc;
-    sample_write_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, w.nug_ridx, w.nug_depth, w.flags, w.pos, m_cap);
+    sample_write_kernel<<<cdiv(m_cap, 256), 256, 0, st>>>(*a, n_live, std_dev, w.nug_ridx, w.nug_depth, w.flags, w.pos, m_cap);
     GSSDF_LAUNCH_OK("sample_write_kernel");
     return GSSDF_OK;
+}
+
+extern "C" int gssdf_sdf_sample_rays(const gssdf_sdf_sample_rays_args *a, gssdf_stream_t stream) { return sample_rays_impl(a, nullptr, nullptr, stream); }
+
+extern "C" int gssdf_sdf_sample_rays_dev(const gssdf_sdf_sample_rays_args *a, const int32_t *n_rays_live, const float *sample_std,
+                                         gssdf_stream_t stream) {
+    return sample_rays_impl(a, n_rays_live, sample_std, stream);
 }
 
 struct GateWs {

@@ -269,7 +269,7 @@ __device__ __forceinline__ bool named_bar_and(int id, int n, bool pred) {
 __device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 __global__ void __launch_bounds__(kFwdTcThreads, 1)
-sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles) {
+sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles, const float *delta_dev) {
     constexpr int TM = 128, HID = 64;
     extern __shared__ __align__(128) unsigned char s_tc[];  // (a larger alignment pads the static part and costs the L1 carve-out step)
     unsigned char *sW = s_tc;                    // 96 KB weight images of all layers (4 x 24 KB), resident
@@ -284,6 +284,7 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nh = 1 + a.net.n_hidden;
     const int64_t n_live = a.n_live ? min((int64_t)*a.n_live, a.n) : a.n;
+    const float delta = delta_dev ? *delta_dev : a.delta;  // gssdf_sdf_fwd_dev: the offset comes from the device
     // A tile holds PT whole points with their V evaluated variants in consecutive rows (row = j * V + v - v0): the six offsets of a
     // point lie within a few cells of each other on the coarse levels, so their corner gathers meet in the same load instruction or
     // in L1 instead of going to L2 six times. skip_base_variant leaves variant 0 out (21 points x 6 + 2 idle rows).
@@ -331,7 +332,7 @@ sdf_fwd_tc_kernel(const gssdf_sdf_fwd_args a, const GridGeom g, int64_t n_tiles)
 #pragma unroll
                 for (int i = 0; i < kFwdEncBatch; ++i) {
                     bool live;
-                    load_x(a.net, a.x, eval_of(tile, (t0 + i * kFwdTcProducers + ptid) % TM, live), a.n, a.delta, x[i]);
+                    load_x(a.net, a.x, eval_of(tile, (t0 + i * kFwdTcProducers + ptid) % TM, live), a.n, delta, x[i]);
                 }
 #pragma unroll
                 for (int i = 0; i < kFwdEncBatch; ++i) f[i] = encode_level<true>(table, g, (t0 + i * kFwdTcProducers + ptid) / TM, x[i]);
@@ -444,7 +445,7 @@ struct TcLossArgs {
 
 template <bool FUSED, bool ANALYTIC>
 __global__ void __launch_bounds__(kBwdTcThreads, 1)
-sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeom g, int64_t n_tiles) {
+sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeom g, int64_t n_tiles, const float *delta_dev) {
     constexpr int TM = 128, HID = 64, NT = kBwdTcThreads;
     extern __shared__ __align__(128) unsigned char s_tc[];  // (a larger alignment pads the static part and costs the L1 carve-out step)
     unsigned char *sF = s_tc;                    // 16 KB a_0: encoded features hi/mid (off_feat); rows 64-127 of its stacked view alias
@@ -472,6 +473,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
     const int nh = 1 + a.net.n_hidden;
     const int64_t n_eval = a.n * max(a.n_variants, 1);
     const int64_t n_live = a.n_live ? min((int64_t)*a.n_live, a.n) : a.n;
+    const float delta = delta_dev ? *delta_dev : a.delta;  // gssdf_sdf_train_dev: the offset comes from the device (a.delta == lo.cfg.delta)
     const __half2 *table = reinterpret_cast<const __half2 *>(a.net.table_half);
     const unsigned char *wimg = reinterpret_cast<const unsigned char *>(a.net.mlp_packed);
     const int V = max(a.n_variants, 1), PT = FUSED ? TM / V : TM;
@@ -618,7 +620,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
             const int c = tid % TM;
             if (c < nc) {
                 float x[3], acc[3] = {0.f, 0.f, 0.f};
-                load_x(a.net, a.x, s_tbase[c / PT] + c % PT, a.n, a.delta, x);
+                load_x(a.net, a.x, s_tbase[c / PT] + c % PT, a.n, delta, x);
 #pragma unroll 1
                 for (int lvl = tid / TM; lvl < kLevels; lvl += NT / TM) {
                     float dx[3] = {0.f, 0.f, 0.f};
@@ -664,7 +666,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
             float r[2] = {0.f, 0.f};
             if (c < nc) {
                 float x[3];
-                load_x(a.net, a.x, s_tbase[c / PT] + c % PT, a.n, a.delta, x);
+                load_x(a.net, a.x, s_tbase[c / PT] + c % PT, a.n, delta, x);
                 encode_level_bwd2(table, a.table_grad, g, lvl, x, gf[c * 33 + 2 * lvl], gf[c * 33 + 2 * lvl + 1], s_cc + c * 3, r);
             }
             __nv_bfloat16 h0, m0, h1, m1;
@@ -749,7 +751,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
             for (int i = 0; i < 4; ++i) {
                 const int task = i * NT + tid, p = task % TM, lvl = task / TM;
                 float x[3];
-                load_x(a.net, a.x, row_gi(p), a.n, a.delta, x);
+                load_x(a.net, a.x, row_gi(p), a.n, delta, x);
                 f[i] = encode_level(table, g, lvl, x);
             }
 #pragma unroll
@@ -837,6 +839,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
                 float sv[7], v_s[7], v_y;
                 for (int v = 0; v < V; ++v) sv[v] = s_out[2 * (tid * V + v)];
                 SdfLossCfg cfg1 = lo.cfg;
+                cfg1.delta = delta;
                 if (analytic) {  // the eikonal / align terms act on the analytic gradient: second-order phase below
                     cfg1.eikonal_weight = 0.f;
                     if (tid == 0) s_tbase[n_coll / PT] = base;  // slots of a batch are filled PT per tile (only a CTA's last tile is partial)
@@ -844,7 +847,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
                         for (int v = 1; v < 7; ++v) sv[v] = __ldg(lo.sdf_variants + (int64_t)v * a.n + i);
                     }
                     if (V == 7 || lo.sdf_variants) {
-                        const float inv2d = 0.5f / lo.cfg.delta;
+                        const float inv2d = 0.5f / delta;
                         s_gnum[(n_coll + tid) * 3 + 0] = (sv[1] - sv[2]) * inv2d;
                         s_gnum[(n_coll + tid) * 3 + 1] = (sv[3] - sv[4]) * inv2d;
                         s_gnum[(n_coll + tid) * 3 + 2] = (sv[5] - sv[6]) * inv2d;
@@ -937,7 +940,7 @@ sdf_bwd_tc_kernel(const gssdf_sdf_bwd_args a, const TcLossArgs lo, const GridGeo
                 const int p = task % TM, lvl = task / TM;
                 if (LIVE_TC(p)) {
                     float x[3], dx[3] = {0.f, 0.f, 0.f};
-                    load_x(a.net, a.x, row_gi(p), a.n, a.delta, x);
+                    load_x(a.net, a.x, row_gi(p), a.n, delta, x);
                     const bool want_dx = a.v_x != nullptr && row_is_base(p);
                     encode_level_bwd(table, a.table_grad, g, lvl, x, gf[p * 33 + 2 * lvl], gf[p * 33 + 2 * lvl + 1], want_dx, dx);
                     if (want_dx) {
@@ -1031,7 +1034,7 @@ static int check_tc(const char *who, const gssdf_sdf_net &net) {
     return GSSDF_OK;
 }
 
-extern "C" int gssdf_sdf_fwd_tc_launch(const gssdf_sdf_fwd_args *a, const gssdf::GridGeom *g, gssdf_stream_t stream) {
+extern "C" int gssdf_sdf_fwd_tc_launch(const gssdf_sdf_fwd_args *a, const gssdf::GridGeom *g, const float *delta_dev, gssdf_stream_t stream) {
     int rc = check_tc("sdf_fwd", a->net);
     if (rc) return rc;
     static bool attr_set = false;
@@ -1045,7 +1048,7 @@ extern "C" int gssdf_sdf_fwd_tc_launch(const gssdf_sdf_fwd_args *a, const gssdf:
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms);
-    sdf_fwd_tc_kernel<<<grid, kFwdTcThreads, kFwdTcSmem, (cudaStream_t)stream>>>(*a, *g, n_tiles);
+    sdf_fwd_tc_kernel<<<grid, kFwdTcThreads, kFwdTcSmem, (cudaStream_t)stream>>>(*a, *g, n_tiles, delta_dev);
     GSSDF_LAUNCH_OK("sdf_fwd_tc_kernel");
     return GSSDF_OK;
 }
@@ -1059,12 +1062,13 @@ extern "C" int gssdf_sdf_bwd_tc_launch(const gssdf_sdf_bwd_args *a, const gssdf:
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms);
-    sdf_bwd_tc_kernel<false, false><<<grid, kBwdTcThreads, bwd_tc_smem(false), (cudaStream_t)stream>>>(*a, TcLossArgs{}, *g, n_tiles);
+    sdf_bwd_tc_kernel<false, false><<<grid, kBwdTcThreads, bwd_tc_smem(false), (cudaStream_t)stream>>>(*a, TcLossArgs{}, *g, n_tiles, nullptr);
     GSSDF_LAUNCH_OK("sdf_bwd_tc_kernel");
     return GSSDF_OK;
 }
 
-extern "C" int gssdf_sdf_train(const gssdf_sdf_train_args *t, gssdf_stream_t stream) {
+// delta_dev: gssdf_sdf_train_dev's device offset (NULL: t->delta, which the host checks)
+static int sdf_train_impl(const gssdf_sdf_train_args *t, const float *delta_dev, gssdf_stream_t stream) {
     GSSDF_REQUIRE(t != nullptr, GSSDF_EINVAL, "sdf_train: null args");
     GSSDF_REQUIRE(t->net.mlp_mode == 1, GSSDF_EUNSUPPORTED, "sdf_train: the fused forward+loss+backward kernel exists for mlp_mode 1 only "
                   "(use gssdf_sdf_fwd + gssdf_sdf_loss + gssdf_sdf_bwd otherwise)");
@@ -1075,7 +1079,7 @@ extern "C" int gssdf_sdf_train(const gssdf_sdf_train_args *t, gssdf_stream_t str
     if (t->n == 0) return GSSDF_OK;
     GSSDF_REQUIRE(t->x && t->net.table_half && t->net.mlp, GSSDF_EINVAL, "sdf_train: x, table_half, mlp must be non-null");
     GSSDF_REQUIRE(t->n_variants == 1 || t->n_variants == 7, GSSDF_EINVAL, "sdf_train: n_variants must be 1 or 7");
-    GSSDF_REQUIRE(t->n_variants == 1 || t->delta > 0.f, GSSDF_EINVAL, "sdf_train: delta must be positive");
+    GSSDF_REQUIRE(delta_dev || t->n_variants == 1 || t->delta > 0.f, GSSDF_EINVAL, "sdf_train: delta must be positive");
     GSSDF_REQUIRE(((uintptr_t)t->table_grad & 7) == 0, GSSDF_EINVAL, "sdf_train: table_grad must be 8-byte aligned");
     gssdf_sdf_bwd_args a{};
     a.net = t->net; a.n = t->n; a.x = t->x; a.n_variants = t->n_variants; a.delta = t->delta; a.n_live = t->n_live;
@@ -1086,7 +1090,7 @@ extern "C" int gssdf_sdf_train(const gssdf_sdf_train_args *t, gssdf_stream_t str
     GSSDF_REQUIRE(t->eikonal_mode == 0 || t->eikonal_mode == 1, GSSDF_EINVAL, "sdf_train: eikonal_mode must be 0 or 1");
     GSSDF_REQUIRE(!(t->eikonal_mode == 1 && t->align_weight > 0.f) || t->n_variants == 7 || t->sdf_variants, GSSDF_EINVAL,
                   "sdf_train: the align loss needs the numerical gradient: n_variants 7 or sdf_variants");
-    GSSDF_REQUIRE(!t->sdf_variants || t->delta > 0.f, GSSDF_EINVAL, "sdf_train: sdf_variants needs the delta they were evaluated with");
+    GSSDF_REQUIRE(delta_dev || !t->sdf_variants || t->delta > 0.f, GSSDF_EINVAL, "sdf_train: sdf_variants needs the delta they were evaluated with");
     GSSDF_REQUIRE(t->eikonal_mode == 1 || t->align_weight == 0.f, GSSDF_EINVAL, "sdf_train: align_weight needs eikonal_mode 1");
     const GridGeom g = make_grid(t->net);
     GSSDF_CUDA_OK(cudaFuncSetAttribute(sdf_bwd_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_tc_smem(false)));
@@ -1098,9 +1102,13 @@ extern "C" int gssdf_sdf_train(const gssdf_sdf_train_args *t, gssdf_stream_t str
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (int)std::min<int64_t>(n_tiles, (int64_t)sms);
     if (t->eikonal_mode == 1)
-        sdf_bwd_tc_kernel<true, true><<<grid, kBwdTcThreads, bwd_tc_smem(true), (cudaStream_t)stream>>>(a, lo, g, n_tiles);
+        sdf_bwd_tc_kernel<true, true><<<grid, kBwdTcThreads, bwd_tc_smem(true), (cudaStream_t)stream>>>(a, lo, g, n_tiles, delta_dev);
     else
-        sdf_bwd_tc_kernel<true, false><<<grid, kBwdTcThreads, bwd_tc_smem(false), (cudaStream_t)stream>>>(a, lo, g, n_tiles);
+        sdf_bwd_tc_kernel<true, false><<<grid, kBwdTcThreads, bwd_tc_smem(false), (cudaStream_t)stream>>>(a, lo, g, n_tiles, delta_dev);
     GSSDF_LAUNCH_OK("sdf_train_kernel");
     return GSSDF_OK;
 }
+
+extern "C" int gssdf_sdf_train(const gssdf_sdf_train_args *t, gssdf_stream_t stream) { return sdf_train_impl(t, nullptr, stream); }
+
+extern "C" int gssdf_sdf_train_dev(const gssdf_sdf_train_args *t, const float *delta, gssdf_stream_t stream) { return sdf_train_impl(t, delta, stream); }

@@ -394,6 +394,58 @@ def sdf_outlier_filter(net, xyz, threshold, columns, n_kept, ws, index=None, n=N
     check(lib().gssdf_sdf_outlier_filter(_lib.C.byref(a), _stream()))
 
 
+def sdf_fwd_dev(net, x, sdf, delta, y1=None, feat=None, n_variants=1, n_live=None, skip_base_variant=False):
+    """sdf_fwd with the offset read from the device: delta = float32 CUDA tensor [1]."""
+    a = make_args("gssdf_sdf_fwd_args", n=x.shape[0], x=x, sdf=sdf, y1=y1, feat=feat, n_variants=n_variants, n_live=n_live,
+                  skip_base_variant=int(bool(skip_base_variant)))
+    a.net = net
+    check(lib().gssdf_sdf_fwd_dev(_lib.C.byref(a), _lib.C.c_void_p(_req(delta, torch.float32, "delta").data_ptr()), _stream()))
+
+
+def sdf_train_dev(net, x, n_variants, delta, gt_sdf, weights, bce_isigma, bce_weight, eikonal_weight, gs_sdf_weight, loss_out,
+                  table_grad=None, mlp_grad=None, v_x=None, visibilities=None, visible_thr=0.0, n_live=None, eikonal_mode=0,
+                  align_weight=0.0, sdf_variants=None, valid_mask=None, n_gate=None):
+    """sdf_train with the offset read from the device: delta = float32 CUDA tensor [1]."""
+    a = make_args("gssdf_sdf_train_args", n=x.shape[0], x=x, n_variants=n_variants, n_live=n_live, gt_sdf=gt_sdf,
+                  weights=weights, visibilities=visibilities, visible_thr=visible_thr, bce_isigma=bce_isigma, bce_weight=bce_weight,
+                  eikonal_weight=eikonal_weight, gs_sdf_weight=gs_sdf_weight, loss_out=loss_out, table_grad=table_grad,
+                  mlp_grad=mlp_grad, v_x=v_x, eikonal_mode=eikonal_mode, align_weight=align_weight,
+                  sdf_variants=sdf_variants, valid_mask=valid_mask, n_gate=n_gate)
+    a.net = net
+    check(lib().gssdf_sdf_train_dev(_lib.C.byref(a), _lib.C.c_void_p(_req(delta, torch.float32, "delta").data_ptr()), _stream()))
+
+
+def sdf_sample_rays_dev(args, n_rays_live=None, sample_std=None):
+    """gssdf_sdf_sample_rays on a filled gssdf_sdf_sample_rays_args (octree.RaySampler builds it) with a device ray count (int32 [1])
+    and a device std (float32 [1]); args.n_rays is the capacity."""
+    nl = _req(n_rays_live, torch.int32, "n_rays_live")
+    sd = _req(sample_std, torch.float32, "sample_std")
+    check(lib().gssdf_sdf_sample_rays_dev(_lib.C.byref(args), _lib.C.c_void_p(nl.data_ptr() if nl is not None else None),
+                                          _lib.C.c_void_p(sd.data_ptr() if sd is not None else None), _stream()))
+
+
+def sdf_ray_batch(pack, rand, n_rays, out, index=None):
+    """Rows i < *n_rays of out = pack rows clamp((int64)(rand[i] * (float)N), 0, N - 1). pack / out: dicts of contiguous CUDA float32
+    origin [.,3], direction [.,3], depth [.] or [.,1], xyz [.,3]; N = pack rows, ray capacity = rand.numel(); n_rays: int32 CUDA [1]."""
+    N = pack["xyz"].shape[0]
+    f32 = torch.float32
+    a = make_args("gssdf_sdf_ray_batch_args", N=N, ray_cap=rand.numel(), rand=_req(rand, f32, "rand"),
+                  n_rays=_req(n_rays, torch.int32, "n_rays"), index=_req(index, torch.int64, "index"),
+                  **{k: _req(pack[k], f32, k) for k in ("origin", "direction", "depth", "xyz")},
+                  **{k + "_out": _req(out[k], f32, k + "_out") for k in ("origin", "direction", "depth", "xyz")})
+    check(lib().gssdf_sdf_ray_batch(_lib.C.byref(a), _stream()))
+
+
+def sdf_adapt(state, y1, n_samples, bce_sigma, bce_isigma, batch_pt_num, update_rays=True):
+    """One nsdf_train / sdf_train_callback state update on the device. state: int32 CUDA [4] holding gssdf_sdf_adapt_state
+    {float sample_std, float pts_per_ray, int32 n_rays, pad} (see nsdf.new_adapt_state); y1: float32 [cap] (variant-0 rows);
+    n_samples: int32 CUDA tensor whose first element is the sample count."""
+    a = make_args("gssdf_sdf_adapt_args", state=_req(state, state.dtype, "state"), y1=_req(y1, torch.float32, "y1"), y1_cap=y1.numel(),
+                  n_samples=_req(n_samples, torch.int32, "n_samples"), bce_sigma=bce_sigma, bce_isigma=bce_isigma,
+                  batch_pt_num=batch_pt_num, update_rays=int(bool(update_rays)))
+    check(lib().gssdf_sdf_adapt(_lib.C.byref(a), _stream()))
+
+
 def scatter_rows3(n, index, n_gate, src, dst, n_live=None):
     a = make_args("gssdf_scatter_rows3_args", n=n, n_live=n_live, index=index, n_gate=n_gate, src=src, dst=dst)
     check(lib().gssdf_scatter_rows3(_lib.C.byref(a), _stream()))

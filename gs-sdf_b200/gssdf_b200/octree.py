@@ -148,7 +148,9 @@ class RaySampler:
         self.rand_free.uniform_()
         self.randn_surface.normal_()
 
-    def sample(self, origin, direction, depth, xyz):
+    def sample(self, origin, direction, depth, xyz, n_live=None, sample_std=None):
+        """n_live (int32 CUDA [1]): only the first *n_live of the n_rays rays are sampled; sample_std (float32 CUDA [1]) replaces the
+        host std. Either one makes this gssdf_sdf_sample_rays_dev, whose results equal the host call on those rays with that std."""
         w = self.ws.buf
         a = make_args("gssdf_sdf_sample_rays_args", n_rays=self.n, origin=origin, direction=direction, depth=depth, xyz=xyz,
                       voxel_sample_num=self.ns, n_free=self.n_free, n_surface=self.n_surf, sample_std=self.std, truncated_dis=self.trunc,
@@ -157,7 +159,10 @@ class RaySampler:
                       out_direction=self.direction, out_depth=self.depth, out_ridx=self.ridx, counts=self.counts, workspace=w,
                       workspace_bytes=w.numel())
         a.tree = self.tree.tree_struct()
-        check(lib().gssdf_sdf_sample_rays(C.byref(a), cabi._stream()))
+        if n_live is None and sample_std is None:
+            check(lib().gssdf_sdf_sample_rays(C.byref(a), cabi._stream()))
+        else:
+            cabi.sdf_sample_rays_dev(a, n_live, sample_std)
         return self.counts
 
 

@@ -190,6 +190,40 @@ def box_room_cull_poses(n, seed=0, radius=0.1, max_yaw=math.radians(50.0), max_p
     return out.astype(np.float32)
 
 
+def box_room_pack(device, n_frames, ds_pt_num=10_000, W=160, H=120, seed=0):
+    """A training depth pack of the BOX room (no pillar) in the layout base_parser.cpp:925-960 builds: per frame `ds_pt_num` pixels drawn
+    without replacement (the per-frame downsampling of k_ds_pt_num), origin = camera centre, unit direction, depth = range along the ray,
+    xyz = direction * depth + origin. Cameras anywhere in the inner half of the room, any yaw, pitch within +-0.8 rad, so every wall,
+    the floor and the ceiling are seen. Returns a dict of float32 tensors on `device`: origin [N,3], direction [N,3], depth [N,1], xyz [N,3].
+    Test and benchmark infrastructure."""
+    import torch
+    rng = np.random.default_rng(seed)
+    c2w = np.zeros((n_frames, 4, 4))
+    for i in range(n_frames):
+        yaw, pitch = rng.uniform(0, 2 * math.pi), rng.uniform(-0.8, 0.8)
+        f = np.array([math.cos(pitch) * math.cos(yaw), math.cos(pitch) * math.sin(yaw), math.sin(pitch)])
+        right = np.cross(f, [0.0, 0.0, 1.0])
+        right /= np.linalg.norm(right)
+        c2w[i, :3, :3] = np.stack([right, np.cross(f, right), f], 1)
+        c2w[i, :3, 3] = rng.uniform(-0.5, 0.5, 3) * BOX
+        c2w[i, 3, 3] = 1.0
+    fx = fy = W / 2.0
+    cx, cy = (W - 1) / 2.0, (H - 1) / 2.0
+    P = torch.from_numpy(c2w).to(device)
+    z = box_room_depth(P.to(torch.float32), fx, fy, cx, cy, W, H, pillar=False)[..., 0].reshape(n_frames, -1).to(torch.float64)
+    k = min(ds_pt_num, W * H)
+    pix = torch.from_numpy(np.stack([rng.choice(W * H, k, replace=False) for _ in range(n_frames)])).to(device)
+    j, i = (pix % W).to(torch.float64), (pix // W).to(torch.float64)
+    dc = torch.stack([(j - cx) / fx, (i - cy) / fy, torch.ones_like(j)], -1)  # [B,k,3] camera ray with z = 1
+    norm = dc.norm(dim=-1, keepdim=True)
+    d = torch.einsum("brc,bkc->bkr", P[:, :3, :3], dc / norm)
+    rng_ = (torch.gather(z, 1, pix) * norm[..., 0])[..., None]
+    o = P[:, None, :3, 3].expand(-1, k, -1)
+    f32 = lambda t: t.reshape(-1, t.shape[-1]).to(torch.float32).contiguous()
+    origin, direction, depth = f32(o), f32(d), f32(rng_)
+    return dict(origin=origin, direction=direction, depth=depth, xyz=(direction * depth + origin).contiguous())
+
+
 def box_room_depth(c2w, fx, fy, cx, cy, W, H, pillar=True, batch=16):
     """Analytic z-depth images [B,H,W,1] float32 of the BOX room's inner walls (plus the occluding pillar) seen from the c2w poses
     [B,4,4] (torch, any device; rendered there `batch` frames at a time), pixel (i, j) along K^-1 [j, i, 1], as the reference's

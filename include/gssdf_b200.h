@@ -1313,6 +1313,77 @@ typedef struct gssdf_sdf_outlier_filter_args {
 size_t gssdf_sdf_outlier_filter_workspace_bytes(int64_t n);
 int gssdf_sdf_outlier_filter(const gssdf_sdf_outlier_filter_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-13  SDF pre-training stage (NeuralSLAM::nsdf_train, include/neural_mapping/neural_mapping.cpp:294-354) without host syncs: the
+ *     quantities the reference reads back with .item() every iteration -- the sample std k_sample_std (also the offset delta of the align
+ *     loss's numerical gradient) and the ray count k_batch_num -- stay on the device (DESIGN 7n). The *_dev entry points take the existing
+ *     argument structs unchanged plus device pointers that override one field each; the non-_dev calls run the same code with NULL. All
+ *     arguments are checked before the first launch; no allocation, no sync.
+ * ------------------------------------------------------------------------------------------ */
+/* sdf_train_batch_iter's batch draw (neural_mapping.cpp:143-156) from a device-resident depth pack (the layout of base_parser.cpp:925-960:
+   unit direction, xyz = direction * depth + origin). For i < min(*n_rays, ray_cap):
+     idx = clamp((int64)(rand[i] * (float)N), 0, N - 1)    (torch's (rand * N).to(kLong).clamp(0, N - 1): N rounds to fp32 as ATen rounds
+                                                            a wrapped scalar; a product of 2^63 or more converts like the CUDA cast)
+     origin_out[i] = origin[idx], direction_out[i] = direction[idx], depth_out[i] = depth[idx], xyz_out[i] = xyz[idx], index[i] = idx.
+   Rows >= *n_rays are untouched. GSSDF_EINVAL for a NULL args / rand / n_rays / pack / output pointer (index may be NULL), N < 1 or
+   ray_cap < 0. */
+typedef struct gssdf_sdf_ray_batch_args {
+    int64_t N;                        /* rows of the pack */
+    const float *origin, *direction;  /* [N,3] */
+    const float *depth;               /* [N] */
+    const float *xyz;                 /* [N,3] */
+    int64_t ray_cap;                  /* capacity of rand and the outputs */
+    const float *rand;                /* [ray_cap] uniform [0,1) */
+    const int32_t *n_rays;            /* device int32: live ray count */
+    float *origin_out, *direction_out; /* [ray_cap,3] */
+    float *depth_out;                 /* [ray_cap] */
+    float *xyz_out;                   /* [ray_cap,3] */
+    int64_t *index;                   /* [ray_cap] or NULL */
+} gssdf_sdf_ray_batch_args;
+int gssdf_sdf_ray_batch(const gssdf_sdf_ray_batch_args *a, gssdf_stream_t stream);
+
+/* gssdf_sdf_sample_rays with a->n_rays as the CAPACITY: only rays i < min(*n_rays_live, a->n_rays) are traced and sampled, and
+   *sample_std (device float) replaces a->sample_std. Every output and count is bit-identical to gssdf_sdf_sample_rays called with
+   n_rays = *n_rays_live and sample_std = *sample_std on the same buffers (the random draws are indexed as there: rand_free[r * n_free + s],
+   randn_surface[r * n_surface + s]). The workspace is sized for the capacity. Either pointer may be NULL (then the struct's field counts). */
+int gssdf_sdf_sample_rays_dev(const gssdf_sdf_sample_rays_args *a, const int32_t *n_rays_live, const float *sample_std, gssdf_stream_t stream);
+
+/* gssdf_sdf_fwd / gssdf_sdf_train with the offset delta read from the device (float) instead of a->delta: every kernel loads it once in
+   its prologue (the variant offsets, and in sdf_train the align loss's 0.5 / delta). Bit-identical to the host-scalar call with the same
+   delta. delta may be NULL (a->delta is used). The host-side `delta > 0` checks do not apply to a device delta: the caller guarantees it
+   is positive and finite (gssdf_sdf_adapt's sample_std is always >= bce_sigma > 0). */
+int gssdf_sdf_fwd_dev(const gssdf_sdf_fwd_args *a, const float *delta, gssdf_stream_t stream);
+int gssdf_sdf_train_dev(const gssdf_sdf_train_args *a, const float *delta, gssdf_stream_t stream);
+
+/* The per-iteration state update of nsdf_train (neural_mapping.cpp:324-330) and sdf_train_callback (:544-548) as one small kernel (one
+   CTA), in the reference's types (params.h:34-36: k_batch_pt_num float, k_batch_num int, k_sample_pts_per_ray float), pt_n = *n_samples:
+     if update_rays:  sample_pts_per_ray = (float)pt_n / (float)n_rays                                     (fp32 IEEE division)
+                      pts_per_ray = (float)((double)pts_per_ray * 0.9 + (double)sample_pts_per_ray * 0.1)  (double, no contraction)
+                      n_rays = (int)min(batch_pt_num / pts_per_ray, batch_pt_num)                      (fp32 division; the min is taken in
+                               float, which equals the reference's min((int)q, (int)batch_pt_num) wherever (int)q is defined)
+     if pt_n > 0:     sample_std = max(mean_{i < pt_n} 1.0f / (1 + softplus_100(y1[i]) * bce_isigma), bce_sigma)
+                      (ATen's softplus, threshold 20; the mean accumulates in fp64 in a fixed order and rounds once: bit-identical from run
+                      to run; the reference's fp32 ATen mean may differ in the last bit)
+   Initial state (params.cpp:198-204, neural_mapping.cpp:298-299): sample_std = bce_sigma, n_rays = (int)batch_pt_num,
+   pts_per_ray = batch_pt_num / (float)n_rays. update_rays = 0 adapts sample_std only (the joint stage's callback).
+   GSSDF_EINVAL for a NULL args / state / n_samples, a NULL y1 with y1_cap > 0, y1_cap < 0, bce_sigma <= 0 or batch_pt_num < 1.
+   pt_n is clamped to y1_cap for the mean. */
+typedef struct gssdf_sdf_adapt_state {
+    float sample_std;                 /* k_sample_std (= the align loss's delta) */
+    float pts_per_ray;                /* k_sample_pts_per_ray */
+    int32_t n_rays;                   /* k_batch_num */
+    int32_t pad;
+} gssdf_sdf_adapt_state;
+typedef struct gssdf_sdf_adapt_args {
+    gssdf_sdf_adapt_state *state;     /* device, updated in place */
+    const float *y1;                  /* [y1_cap] raw decoder output 1 of the step's samples (variant-0 rows) */
+    int64_t y1_cap;
+    const int32_t *n_samples;         /* device int32: pt_n (counts[0] of gssdf_sdf_sample_rays) */
+    float bce_sigma, bce_isigma, batch_pt_num;
+    int32_t update_rays;              /* 1: EMA + ray count (nsdf_train); 0: sample_std only */
+} gssdf_sdf_adapt_args;
+int gssdf_sdf_adapt(const gssdf_sdf_adapt_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
