@@ -29,8 +29,9 @@ struct AdamPlan {
     int8_t rowg[GSSDF_ADAM_MAX_ROW_GROUPS];          // args.groups index of row group k
     int32_t n_dense, n_rowg, row_width;              // row_width = summed widths of the row groups
     int64_t n_rows;                                  // rows of every row group
-    float step_size[GSSDF_ADAM_MAX_GROUPS];          // lr / (1 - beta1^t)
-    float inv_sqrt_bc2;                              // 1 / sqrt(1 - beta2^t)
+    float step_size[GSSDF_ADAM_MAX_GROUPS];          // lr / (1 - beta1^t), t = the group's step
+    float inv_sqrt_bc2[GSSDF_ADAM_MAX_GROUPS];       // 1 / sqrt(1 - beta2^t), t = the group's step
+    int32_t row_step;                                // the step every row group takes (they share one clock)
 };
 
 // Rows [blk * kAdamRowsPerCta, +kAdamRowsPerCta) of the visit list; a row's parameters are consecutive threads, the row groups side by
@@ -39,7 +40,7 @@ __device__ __forceinline__ void adam_rows(const gssdf_adam_args &a, const AdamPl
     const int64_t n = a.row_ids ? min((int64_t)a.row_count->nnz, (int64_t)a.row_cap) : plan.n_rows;
     const int64_t k0 = blk * kAdamRowsPerCta;
     if (k0 >= n) return;  // CTA-uniform
-    const int t = a.step, rw = plan.row_width, w0 = a.groups[plan.rowg[0]].row_width;
+    const int t = plan.row_step, rw = plan.row_width, w0 = a.groups[plan.rowg[0]].row_width;
     const float b1 = a.beta1, b2 = a.beta2, eps = a.eps, gs = a.grad_scale;
     for (int e = threadIdx.x; e < kAdamRowsPerCta * rw; e += kAdamThreads) {
         const int kr = e / rw, c = e - kr * rw;
@@ -55,7 +56,7 @@ __device__ __forceinline__ void adam_rows(const gssdf_adam_args &a, const AdamPl
             adam_replay(p, m, v, from, t, r, gk);
         } else {
             adam_replay(p, m, v, from, t - 1, r, gk);
-            adam_one(p, a.grads[i], m, v, b1, b2, eps, gs, plan.step_size[plan.rowg[gk]], plan.inv_sqrt_bc2);
+            adam_one(p, a.grads[i], m, v, b1, b2, eps, gs, plan.step_size[plan.rowg[gk]], plan.inv_sqrt_bc2[plan.rowg[gk]]);
             if (a.zero_grads) a.grads[i] = 0.f;
         }
         a.params[i] = p; a.exp_avg[i] = m; a.exp_avg_sq[i] = v;
@@ -78,7 +79,7 @@ __global__ void __launch_bounds__(kAdamThreads) adam_kernel(const gssdf_adam_arg
     const int gi = plan.dense[di];
     const gssdf_adam_group grp = a.groups[gi];
     const int64_t chunk0 = (int64_t)(blockIdx.x - plan.first_block[di]) * kAdamChunk;
-    const float b1 = a.beta1, b2 = a.beta2, eps = a.eps, gs = a.grad_scale, ss = plan.step_size[gi], isb2 = plan.inv_sqrt_bc2;
+    const float b1 = a.beta1, b2 = a.beta2, eps = a.eps, gs = a.grad_scale, ss = plan.step_size[gi], isb2 = plan.inv_sqrt_bc2[gi];
     float *P = a.params + grp.offset, *G = a.grads + grp.offset, *M = a.exp_avg + grp.offset, *V = a.exp_avg_sq + grp.offset;
     __half *Hs = (grp.half_shadow && a.table_half) ? reinterpret_cast<__half *>(a.table_half) : nullptr;
     const bool vec = ((grp.offset & 3) == 0);  // cudaMalloc'ed bases are 256-byte aligned: the slice is float4-aligned iff its offset is
@@ -171,27 +172,34 @@ extern "C" int gssdf_adam_replay_push(gssdf_adam_replay *r, int32_t step, float 
     return GSSDF_OK;
 }
 
-extern "C" int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream) {
+// group_steps: the step of each group (host array of n_groups), or NULL for every group at a->step.
+static int adam_launch(const gssdf_adam_args *a, const int32_t *group_steps, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "adam_step: null args");
     GSSDF_REQUIRE(a->params && a->grads && a->exp_avg && a->exp_avg_sq, GSSDF_EINVAL, "adam_step: null buffer");
     GSSDF_REQUIRE(a->n_groups >= 0 && a->n_groups <= GSSDF_ADAM_MAX_GROUPS, GSSDF_EINVAL, "adam_step: n_groups out of range");
-    GSSDF_REQUIRE(a->step >= 1, GSSDF_EINVAL, "adam_step: step must be >= 1");
+    GSSDF_REQUIRE(group_steps || a->step >= 1, GSSDF_EINVAL, "adam_step: step must be >= 1");
     GSSDF_REQUIRE(a->beta1 >= 0.f && a->beta1 < 1.f && a->beta2 >= 0.f && a->beta2 < 1.f && a->eps >= 0.f, GSSDF_EINVAL, "adam_step: bad betas / eps");
     AdamPlan plan{};
     int64_t blocks = 0;
-    double bc1, bc2;
-    adam_bias_corrections(a->beta1, a->beta2, a->step, bc1, bc2);
     plan.n_rows = -1;
+    plan.row_step = -1;
     for (int gi = 0; gi < a->n_groups; ++gi) {
         const gssdf_adam_group &g = a->groups[gi];
+        const int32_t t = group_steps ? group_steps[gi] : a->step;
+        GSSDF_REQUIRE(t >= 1, GSSDF_EINVAL, "adam_step: group %d has step %d < 1", gi, t);
         GSSDF_REQUIRE(g.offset >= 0 && g.count >= 0 && g.row_width >= 0, GSSDF_EINVAL, "adam_step: bad group %d", gi);
         GSSDF_REQUIRE(!g.half_shadow || a->table_half, GSSDF_EINVAL, "adam_step: group %d wants a half shadow but table_half is null", gi);
+        double bc1, bc2;
+        adam_bias_corrections(a->beta1, a->beta2, t, bc1, bc2);
         plan.step_size[gi] = adam_step_size(g.lr, bc1);
+        plan.inv_sqrt_bc2[gi] = adam_inv_sqrt_bc2(bc2);
         if (g.row_width > 0) {
             GSSDF_REQUIRE(plan.n_rowg < GSSDF_ADAM_MAX_ROW_GROUPS && !g.half_shadow && g.count % g.row_width == 0, GSSDF_EINVAL,
                           "adam_step: bad row group %d", gi);
             GSSDF_REQUIRE(plan.n_rows < 0 || plan.n_rows == g.count / g.row_width, GSSDF_EINVAL, "adam_step: row groups differ in rows");
+            GSSDF_REQUIRE(plan.row_step < 0 || plan.row_step == t, GSSDF_EINVAL, "adam_step: row groups differ in step (%d, %d)", plan.row_step, t);
             plan.n_rows = g.count / g.row_width;
+            plan.row_step = t;
             plan.row_width += g.row_width;
             plan.rowg[plan.n_rowg++] = (int8_t)gi;
             continue;
@@ -203,10 +211,10 @@ extern "C" int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream) 
         GSSDF_REQUIRE(blocks < (int64_t)1 << 31, GSSDF_EINVAL, "adam_step: too many parameters for one launch");
     }
     plan.first_block[plan.n_dense] = (int32_t)blocks;
-    plan.inv_sqrt_bc2 = adam_inv_sqrt_bc2(bc2);
     gssdf_adam_replay r{};
     if (plan.n_rowg > 0 && plan.n_rows > 0) {
-        GSSDF_REQUIRE(a->replay && a->replay->last && a->replay->step == a->step, GSSDF_EINVAL, "adam_step: row groups need replay (step %d)", a->step);
+        GSSDF_REQUIRE(a->replay && a->replay->last && a->replay->step == plan.row_step, GSSDF_EINVAL, "adam_step: row groups need replay (step %d)",
+                      plan.row_step);
         GSSDF_REQUIRE(a->replay->beta1 == a->beta1 && a->replay->beta2 == a->beta2 && a->replay->eps == a->eps && a->grad_scale > 0.f,
                       GSSDF_EINVAL, "adam_step: replay constants differ from the step's, or grad_scale <= 0");
         GSSDF_REQUIRE(!a->row_ids || (a->row_count && a->row_cap >= 0), GSSDF_EINVAL, "adam_step: row_ids without row_count / row_cap");
@@ -221,6 +229,13 @@ extern "C" int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream) 
     }
     if (a->net && a->mlp_packed) return gssdf_sdf_mlp_pack(a->net, a->mlp_packed, stream);
     return GSSDF_OK;
+}
+
+extern "C" int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream) { return adam_launch(a, nullptr, stream); }
+
+extern "C" int gssdf_adam_step_clocks(const gssdf_adam_args *a, const int32_t *group_steps, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(group_steps != nullptr, GSSDF_EINVAL, "adam_step_clocks: null group_steps");
+    return adam_launch(a, group_steps, stream);
 }
 
 extern "C" int gssdf_isotropic_loss(const gssdf_isotropic_loss_args *a, gssdf_stream_t stream) {

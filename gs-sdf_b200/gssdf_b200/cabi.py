@@ -328,11 +328,8 @@ class AdamReplay:
         return _lib.C.addressof(self.s)
 
 
-def adam_step(params, grads, exp_avg, exp_avg_sq, groups, step, beta1=0.9, beta2=0.999, eps=1e-15, grad_scale=1.0, zero_grads=True,
-              table_half=None, net=None, mlp_packed=None, replay=None, row_ids=None, row_count=None, row_cap=0, replay_only=False):
-    """groups: list of (offset, count, lr, half_shadow[, row_width]). `net` (gssdf_sdf_net struct, kept alive by the caller) + mlp_packed:
-    re-pack the decoder's bf16 operand image after the update. Row groups (row_width > 0) need `replay` (AdamReplay, pushed for `step`);
-    row_ids + row_count (device counts, ->nnz) + row_cap: visit those rows only, else every row (see gssdf_adam_args)."""
+def _adam_args(params, grads, exp_avg, exp_avg_sq, groups, step, beta1=0.9, beta2=0.999, eps=1e-15, grad_scale=1.0, zero_grads=True,
+               table_half=None, net=None, mlp_packed=None, replay=None, row_ids=None, row_count=None, row_cap=0, replay_only=False):
     a = make_args("gssdf_adam_args", params=params, grads=grads, exp_avg=exp_avg, exp_avg_sq=exp_avg_sq, n_groups=len(groups), step=step,
                   beta1=beta1, beta2=beta2, eps=eps, grad_scale=grad_scale, zero_grads=int(bool(zero_grads)), table_half=table_half,
                   mlp_packed=mlp_packed, replay=replay.ptr() if replay is not None else None, row_ids=row_ids, row_count=row_count,
@@ -343,7 +340,25 @@ def adam_step(params, grads, exp_avg, exp_avg_sq, groups, step, beta1=0.9, beta2
         a.groups[i].row_width = int(grp[4]) if len(grp) > 4 else 0
     if net is not None:
         a.net = _lib.C.cast(_lib.C.pointer(net), _lib.C.c_void_p)
-    check(lib().gssdf_adam_step(_lib.C.byref(a), _stream()))
+    return a
+
+
+def adam_step(params, grads, exp_avg, exp_avg_sq, groups, step, **kw):
+    """groups: list of (offset, count, lr, half_shadow[, row_width]). `net` (gssdf_sdf_net struct, kept alive by the caller) + mlp_packed:
+    re-pack the decoder's bf16 operand image after the update. Row groups (row_width > 0) need `replay` (AdamReplay, pushed for `step`);
+    row_ids + row_count (device counts, ->nnz) + row_cap: visit those rows only, else every row (see gssdf_adam_args). Keywords: beta1,
+    beta2, eps, grad_scale, zero_grads, table_half, net, mlp_packed, replay, row_ids, row_count, row_cap, replay_only."""
+    check(lib().gssdf_adam_step(_lib.C.byref(_adam_args(params, grads, exp_avg, exp_avg_sq, groups, step, **kw)), _stream()))
+
+
+def adam_step_clocks(params, grads, exp_avg, exp_avg_sq, groups, steps, **kw):
+    """adam_step with one step per group (`steps`, a sequence as long as `groups`; the row groups share one step, for which `replay` is
+    pushed): gssdf_adam_step_clocks."""
+    if len(steps) != len(groups):
+        raise ValueError(f"gssdf_b200: {len(steps)} steps for {len(groups)} groups")
+    a = _adam_args(params, grads, exp_avg, exp_avg_sq, groups, 1, **kw)
+    st = (_lib.C.c_int32 * max(len(steps), 1))(*[int(t) for t in steps])
+    check(lib().gssdf_adam_step_clocks(_lib.C.byref(a), _lib.C.cast(st, _lib.C.c_void_p), _stream()))
 
 
 def _rows_args(segments, cap_rows, n_rows, row_ids, flat, packed, zero_source=False):

@@ -196,15 +196,17 @@ class SdfTrainer:
         if self.outlier_remove and i > 0 and i % self.outlier_interval == 0:
             self.remove_outliers(i)
 
-    def remove_outliers(self, i):
+    def remove_outliers(self, i, total_iter=None, net=None, outlier_dist=None):
         """sdf_train_callback's outlier branch on the device pack (sdf.remove_outliers' rule: threshold and rows from sdf.outlier_threshold /
-        sdf.outlier_rows, compaction by gssdf_sdf_outlier_filter into the second pack buffer). Reads the kept count once."""
-        thr = SD.outlier_threshold(i, self.iters, self.truncated_dis, self.outlier_dist)
+        sdf.outlier_rows, compaction by gssdf_sdf_outlier_filter into the second pack buffer). Reads the kept count once. total_iter / net /
+        outlier_dist default to this stage's; the joint stage (gstrain) passes its iteration count, its SDF and its setting."""
+        thr = SD.outlier_threshold(i, self.iters if total_iter is None else total_iter, self.truncated_dis,
+                                   self.outlier_dist if outlier_dist is None else outlier_dist)
         n = SD.outlier_rows(self.N, self.vis_batch_pt_num)
         if self._pack_alt is None:
             self._pack_alt = {k: torch.empty_like(v) for k, v in self._pack.items()}
         cols = [(self._pack[k], self._pack_alt[k]) for k in PACK_KEYS]
-        cabi.sdf_outlier_filter(self.net, self._pack["xyz"], thr, cols, self.n_kept, self.ws, n=n)
+        cabi.sdf_outlier_filter(self.net if net is None else net, self._pack["xyz"], thr, cols, self.n_kept, self.ws, n=n)
         kept = int(self.n_kept.item())
         if kept < 1:
             raise RuntimeError(f"SdfTrainer: the outlier removal of iteration {i} (threshold {thr:g}) kept no row of the pack")

@@ -104,9 +104,10 @@ class SplatRenderer:
 
     # -- loss + backward -----------------------------------------------------------------------
     def backward(self, means, quats, scales, opacities, sh, viewmats, Ks, gt, randns=None, w_rgb=1.0, w_depth=0.1, v_samples=None,
-                 zero_grads=True, raw=None, w_dssim=0.0, w_normal=0.0, w_isotropic=0.0, before_projection_bwd=None):
+                 zero_grads=True, raw=None, w_dssim=0.0, w_normal=0.0, w_isotropic=0.0, before_projection_bwd=None, projection_bwd=True):
         """With raw parameters the flat gradient holds dL/d(offsets|quats|log-scales|logits|features_dc|features_rest); the SH segment
-        keeps its [N,K,3] size, laid out as dc [N,1,3] followed by rest [N,K-1,3]."""
+        keeps its [N,K,3] size, laid out as dc [N,1,3] followed by rest [N,K-1,3]. projection_bwd=False stops after the SH backward (the
+        structure is frozen: only the colour gradient is wanted)."""
         C, W, H, cap = self.C, self.W, self.H, self.cap
         off, rest = (raw["offsets"], raw["sh_rest"]) if raw else (None, None)
         N, K = self.N, self.K
@@ -144,6 +145,8 @@ class SplatRenderer:
                              self.p["gaussian_ids"], self.p["radii"], self.colors, self.g["v_colors"], v_sh, self.v_means,
                              mean_offsets=off, sh_rest=rest, v_sh_rest=v_rest)
         self._mark("sh_bwd")
+        if not projection_bwd:
+            return self.loss
         if before_projection_bwd is not None:  # v_samples may be produced on another stream (GsSdfStep.overlap)
             before_projection_bwd()
         cabi.project2dgs_bwd(means, quats, scales, viewmats, Ks, W, H, cap, self.counts, self.p["camera_ids"],
@@ -186,7 +189,9 @@ class GsSdfStep:
     def __init__(self, N, K, W, H, device, isect_cap, sdf_net_cfg, n_ray_samples=32768, sh_degree=3, origin=(0.0, 0.0, 0.0),
                  map_size=14.0, bce_sigma=0.1, delta=None, eikonal_weight=0.1, gs_sdf_weight=1e-3, visible_thr=0.1, mlp_mode=None,
                  eikonal_mode=None, align_weight=0.1, rgb_weight=0.8, dssim_weight=0.2, depth_weight=0.1, normal_weight=0.0,
-                 isotropic_weight=0.0):
+                 isotropic_weight=0.0, delta_dev=None):
+        """delta_dev: float32 CUDA tensor [1] read by every SDF call of [A] and [C] in place of the host scalar `delta` (the sample std the
+        SDF stage adapts on the device, nsdf.SdfTrainer.std_dev); the ray-site forward then also evaluates the base variant into ray_y1."""
         self.R = SplatRenderer(N, K, 1, W, H, device, isect_cap, sh_degree=sh_degree)
         self.dev, self.N, self.n_ray = device, N, n_ray_samples
         self.cfg = dict(sdf_net_cfg)
@@ -213,6 +218,12 @@ class GsSdfStep:
         self.eik_mode = (1 if self.mlp_mode == 1 else 0) if eikonal_mode is None else int(eikonal_mode)
         assert self.eik_mode == 0 or self.mlp_mode == 1, "the analytic eikonal path lives in the fused tensor-core kernel (mlp_mode 1)"
         self.align_w = float(align_weight) if self.eik_mode == 1 else 0.0
+        if delta_dev is not None:
+            if self.eik_mode != 1:
+                raise ValueError("GsSdfStep: a device delta needs eikonal_mode 1 (the numerical-gradient path has no device-delta entry)")
+            if not (isinstance(delta_dev, torch.Tensor) and delta_dev.is_cuda and delta_dev.dtype == torch.float32 and delta_dev.numel() == 1):
+                raise ValueError("GsSdfStep: delta_dev must be a float32 CUDA tensor [1]")
+        self.delta_dev = delta_dev
         # flat gradient: [splat | (pad to an even offset: the table gradient takes 8-byte vector REDs) | table | mlp]
         n_splat = self.R.flat_grad.numel()
         t0 = (n_splat + 1) // 2 * 2
@@ -288,7 +299,13 @@ class GsSdfStep:
         cabi.sdf_gate_compact(cap, samples, self.gate_idx, self.gate_x, self.n_gate, self.gate_ws, visibilities=R.r["visibilities"],
                               visible_thr=self.vis_thr, valid_mask=self.valid_mask, weights=R.p["sample_weights"], w_out=self.gate_w,
                               n_live=n_live)
-        if self.eik_mode == 1:
+        if self.eik_mode == 1 and self.delta_dev is not None:
+            if self.align_w > 0:
+                cabi.sdf_fwd_dev(net, self.gate_x, self.gs_sdf, self.delta_dev, n_variants=7, n_live=self.n_gate, skip_base_variant=True)
+            cabi.sdf_train_dev(net, self.gate_x, 1, self.delta_dev, None, self.gate_w, self.bce_isigma, 0.0, self.eik_w, self.gs_sdf_w,
+                               self.sdf_loss, self.table_grad, self.mlp_grad, self.gate_vx, n_live=self.n_gate, eikonal_mode=1,
+                               align_weight=self.align_w, sdf_variants=self.gs_sdf if self.align_w > 0 else None)
+        elif self.eik_mode == 1:
             if self.align_w > 0:
                 cabi.sdf_fwd(net, self.gate_x, self.gs_sdf, None, None, n_variants=7, delta=self.delta, n_live=self.n_gate,
                              skip_base_variant=True)
@@ -305,7 +322,8 @@ class GsSdfStep:
 
     def step(self, scene, table_f32, mlp, viewmats, Ks, gt_image, ray_xyz, ray_gt_sdf, randns=None, on_sdf_grads_ready=None,
              before_render=None, ray_n_live=None):
-        """ray_n_live: device int32 (e.g. RaySampler.counts): only the first *ray_n_live rows of ray_xyz / ray_gt_sdf are samples."""
+        """ray_n_live: device int32 (e.g. RaySampler.counts): only the first *ray_n_live rows of ray_xyz / ray_gt_sdf are samples.
+        ray_xyz None: no SDF stage [A] (detach_sdf_grad: the SDF is frozen)."""
         """Hooks for a data-parallel caller (both optional):
         on_sdf_grads_ready(table_and_mlp_grad): the hash-table / decoder gradients are final (after [C]) -> start reducing them while the
             render backward [D] is still running.
@@ -327,7 +345,15 @@ class GsSdfStep:
                 self.flat_grad[t0:].zero_()  # table + decoder segment; the splat segment is cleared after before_render()
             self.sdf_loss.zero_()
             # [A] SDF stage on the ray samples (tensor-core mode: forward + losses + backward fused in one kernel)
-            if self.mlp_mode == 1:
+            if ray_xyz is None:
+                pass
+            elif self.delta_dev is not None:  # base variant included: y1 of the base rows feeds the sample-std update (gssdf_sdf_adapt)
+                cabi.sdf_fwd_dev(net, ray_xyz, self.ray_sdf, self.delta_dev, y1=self.ray_y1, n_variants=7 if self.align_w > 0 else 1,
+                                 n_live=ray_n_live)
+                cabi.sdf_train_dev(net, ray_xyz, 1, self.delta_dev, ray_gt_sdf, None, self.bce_isigma, 1.0, self.eik_w, 0.0, self.sdf_loss,
+                                   self.table_grad, self.mlp_grad, None, eikonal_mode=1, align_weight=self.align_w,
+                                   sdf_variants=self.ray_sdf if self.align_w > 0 else None, n_live=ray_n_live)
+            elif self.mlp_mode == 1:
                 if self.eik_mode == 1:  # reference default: forward-only pass over the 7 variants (numerical gradient of the align loss),
                                         # then forward + losses + backward + double backward on the base points only
                     if self.align_w > 0:
@@ -378,7 +404,14 @@ class GsSdfStep:
         cabi.sdf_gate_count(cap, self.n_gate, visibilities=R.r["visibilities"], visible_thr=self.vis_thr, valid_mask=self.valid_mask,
                             n_live=n_live)
         gate = dict(valid_mask=self.valid_mask, n_gate=self.n_gate)
-        if self.mlp_mode == 1:
+        if self.mlp_mode == 1 and self.delta_dev is not None:
+            if self.align_w > 0:
+                cabi.sdf_fwd_dev(net, samples, self.gs_sdf, self.delta_dev, n_variants=7, n_live=n_live, skip_base_variant=True)
+            cabi.sdf_train_dev(net, samples, 1, self.delta_dev, None, R.p["sample_weights"], self.bce_isigma, 0.0, self.eik_w, self.gs_sdf_w,
+                               self.sdf_loss, self.table_grad, self.mlp_grad, self.v_samples, visibilities=R.r["visibilities"],
+                               visible_thr=self.vis_thr, n_live=n_live, eikonal_mode=1, align_weight=self.align_w,
+                               sdf_variants=self.gs_sdf if self.align_w > 0 else None, **gate)
+        elif self.mlp_mode == 1:
             if self.eik_mode == 1:
                 if self.align_w > 0:
                     cabi.sdf_fwd(net, samples, self.gs_sdf, None, None, n_variants=7, delta=self.delta, n_live=n_live, skip_base_variant=True)
@@ -451,6 +484,7 @@ class GsSdfTrainer(GsSdfStep):
         self.anchors_buf = torch.zeros(N, 3, **f32)
         self.keep_shadows = True
         self.t_splat = self.t_sdf = 0
+        self.t_sh = 0  # the SH groups' Adam step: t_splat unless colour initialisation stepped them alone (adam_sh)
         self._net = None
         self.l2_persist = False  # off by default: the 30.5 MB table fits the 50 MB L2 without a persistence window
         self.N_cap = N
@@ -486,11 +520,11 @@ class GsSdfTrainer(GsSdfStep):
         self._exp_avg_sq = t
 
     def flush_sh(self):
-        """Replay the skipped zero-gradient Adam steps of every stale SH row up to t_splat (one launch; nothing when all are current)."""
+        """Replay the skipped zero-gradient Adam steps of every stale SH row up to t_sh (one launch; nothing when all are current)."""
         if not self._sh_stale:
             return
         self._sh_stale = False
-        cabi.adam_step(self._params, self.flat_grad, self._exp_avg, self._exp_avg_sq, self._sh_groups(), self.t_splat,
+        cabi.adam_step(self._params, self.flat_grad, self._exp_avg, self._exp_avg_sq, self._sh_groups(), self.t_sh,
                        replay=self.sh_replay, replay_only=True)
 
     def _sh_groups(self):
@@ -499,14 +533,14 @@ class GsSdfTrainer(GsSdfStep):
 
     def _sh_catch_up(self):
         """Before the SH forward reads them: the rows of this step's camera get the zero-gradient steps they missed (one launch)."""
-        if self.t_splat > 0:
-            cabi.adam_step(self._params, self.flat_grad, self._exp_avg, self._exp_avg_sq, self._sh_groups(), self.t_splat,
+        if self.t_sh > 0:
+            cabi.adam_step(self._params, self.flat_grad, self._exp_avg, self._exp_avg_sq, self._sh_groups(), self.t_sh,
                            replay=self.sh_replay, row_ids=self.R.p["gaussian_ids"], row_count=self.R.counts, row_cap=self.R.cap,
                            replay_only=True)
 
     def stamp_sh_current(self):
-        """Every SH row holds its values at step t_splat (after load / a row remap of current rows)."""
-        self.sh_last.fill_(self.t_splat)
+        """Every SH row holds its values at step t_sh (after load / a row remap of current rows)."""
+        self.sh_last.fill_(self.t_sh)
         self._sh_stale = False
 
     def set_live(self, n_live):
@@ -525,13 +559,19 @@ class GsSdfTrainer(GsSdfStep):
         # (offset, count, lr, half_shadow, row_width): features_dc / features_rest are row groups on the lazy path
         self.splat_groups = [(o[i], n * w[i], self.lr[i], False, w[i] if (self.lazy_sh and i >= 4) else 0)
                              for i in range(6) if w[i] > 0 and n > 0]
+        self.splat_group_is_sh = [i >= 4 for i in range(6) if w[i] > 0 and n > 0]
         t0 = self.t0
         self.sdf_groups = [(t0, self.n_table, self.sdf_lr, True), (t0 + self.n_table, self.n_mlp, self.sdf_lr, False)]
         self.table, self.mlp = pv[t0:t0 + self.n_table], pv[t0 + self.n_table:]
         if self._net is not None:
             self._net = cabi.sdf_net(self.table_half, self.mlp, **self.cfg)
 
-    def load(self, anchors, offsets, quats, log_scales, logit_opacities, features_dc, features_rest, table, mlp):
+    def load(self, anchors, offsets, quats, log_scales, logit_opacities, features_dc, features_rest, table, mlp, sdf_exp_avg=None,
+             sdf_exp_avg_sq=None, sdf_step=0):
+        """sdf_exp_avg / sdf_exp_avg_sq ([table | decoder], e.g. nsdf.SdfTrainer's) and sdf_step: the SDF groups continue with those Adam
+        moments and that step count (one optimiser spans both stages in the reference); without them the SDF moments start at zero."""
+        if (sdf_exp_avg is None) != (sdf_exp_avg_sq is None) or (sdf_exp_avg is None and sdf_step != 0) or sdf_step < 0:
+            raise ValueError("GsSdfTrainer.load: give both SDF moments with their step count, or neither")
         self.set_live(anchors.shape[0])
         sc = self.scene
         self.anchors.copy_(anchors)
@@ -541,7 +581,12 @@ class GsSdfTrainer(GsSdfStep):
             sc["raw"]["sh_rest"].copy_(features_rest)
         self.table.copy_(table); self.mlp.copy_(mlp)
         self._exp_avg.zero_(); self._exp_avg_sq.zero_(); self.flat_grad.zero_()
-        self.t_splat = self.t_sdf = 0
+        self.t_splat = self.t_sdf = self.t_sh = 0
+        if sdf_exp_avg is not None:
+            n_sdf = self.n_table + self.n_mlp
+            self._exp_avg[self.t0:self.t0 + n_sdf].copy_(sdf_exp_avg.reshape(-1))
+            self._exp_avg_sq[self.t0:self.t0 + n_sdf].copy_(sdf_exp_avg_sq.reshape(-1))
+            self.t_sdf = int(sdf_step)
         self.stamp_sh_current()
         cabi.sdf_table_to_half(self.table, self.table_half)
         self._net = cabi.sdf_net(self.table_half, self.mlp, **self.cfg)
@@ -560,7 +605,8 @@ class GsSdfTrainer(GsSdfStep):
 
     def _next_splat_step(self):
         self.t_splat += 1
-        self.sh_replay.push(self.t_splat, self.lr[4], self.lr[5])
+        self.t_sh += 1
+        self.sh_replay.push(self.t_sh, self.lr[4], self.lr[5])
         return self.t_splat
 
     def adam_sdf(self, grad_scale=1.0):
@@ -579,7 +625,7 @@ class GsSdfTrainer(GsSdfStep):
         saw (the only rows with an SH gradient) and sweep every row once per ADAM_WINDOW steps, so that no row falls a window behind."""
         self.t_sdf += 1
         t = self._next_splat_step()
-        assert self.t_sdf == t
+        assert self.t_sdf == t == self.t_sh
         self._adam_call(self.splat_groups + self.sdf_groups, t, grad_scale, True, rows=self.lazy_sh and not sh_sweep_step(t))
         self.R._mark("adam")
 
@@ -587,3 +633,50 @@ class GsSdfTrainer(GsSdfStep):
                    ray_n_live=None):
         return self.step(self.scene, self.table, self.mlp, viewmats, Ks, gt_image, ray_xyz, ray_gt_sdf, randns,
                          on_sdf_grads_ready=on_sdf_grads_ready, before_render=before_render, ray_n_live=ray_n_live)
+
+    # ---- per-group clocks (gstrain.GsTrainer: the SDF groups arrive with the SDF stage's steps, the SH groups with colour
+    # initialisation's) -------------------------------------------------------------------------------------------------------------
+    def adam_clocks(self, sdf=True):
+        """adam_all with every group at its own step count: SDF groups t_sdf + 1, SH groups t_sh + 1, the other splat groups t_splat + 1
+        (gssdf_adam_step_clocks, one launch). sdf=False leaves the SDF groups out (detach_sdf_grad)."""
+        t = self._next_splat_step()
+        steps = [self.t_sh if is_sh else t for is_sh in self.splat_group_is_sh]
+        groups = list(self.splat_groups)
+        if sdf:
+            self.t_sdf += 1
+            groups += self.sdf_groups
+            steps += [self.t_sdf] * len(self.sdf_groups)
+        self._adam_clocks_call(groups, steps, sdf, rows=self.lazy_sh and not sh_sweep_step(self.t_sh))
+        self.R._mark("adam")
+
+    def adam_sh(self):
+        """Adam over the SH groups alone at the next SH step (colour initialisation: the structure and the SDF are frozen)."""
+        self.t_sh += 1
+        self.sh_replay.push(self.t_sh, self.lr[4], self.lr[5])
+        groups = [g for g, is_sh in zip(self.splat_groups, self.splat_group_is_sh) if is_sh]
+        self._adam_clocks_call(groups, [self.t_sh] * len(groups), False, rows=self.lazy_sh and not sh_sweep_step(self.t_sh))
+
+    def _adam_clocks_call(self, groups, steps, sdf, rows):
+        row = dict(row_ids=self.R.p["gaussian_ids"], row_count=self.R.counts, row_cap=self.R.cap) if rows else {}
+        cabi.adam_step_clocks(self._params, self.flat_grad, self._exp_avg, self._exp_avg_sq, groups, steps, zero_grads=True,
+                              table_half=self.table_half if sdf else None, net=self._net if (sdf and self.mlp_mode == 1) else None,
+                              mlp_packed=self.mlp_packed if (sdf and self.mlp_mode == 1) else None, replay=self.sh_replay, **row)
+        self._sh_stale = rows
+
+    def color_step(self, viewmats, Ks, gt_image):
+        """One colour-initialisation iteration (gs_train_batch_iter(i, false) + Adam, neural_mapping.cpp:377-382): render at the current
+        SH degree, the photometric loss alone (L1 + DSSIM: no SDF stage, no coupling, no normal, depth or isotropic term), the backward
+        down to the SH coefficients (the frozen structure's projection backward is skipped) and Adam over the SH groups. The structure's
+        gradient segments are left for the caller to clear."""
+        R, sc = self.R, self.scene
+        R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], viewmats, Ks, raw=sc["raw"])
+        loss = R.backward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], viewmats, Ks, gt_image, zero_grads=False,
+                          raw=sc["raw"], w_rgb=self.rgb_w, w_depth=0.0, w_dssim=self.dssim_w, projection_bwd=False)
+        self.adam_sh()
+        return loss
+
+    def sdf_net(self):
+        """The gssdf_sdf_net of the current SDF (fp16 table shadow and decoder image as the optimiser keeps them), for operators run
+        between steps (outlier removal)."""
+        return cabi.sdf_net(self.table_half, self.mlp, origin=self.origin, inv_size=self.inv_size, mlp_mode=self.mlp_mode,
+                            mlp_packed=self.mlp_packed, **self.cfg)

@@ -253,3 +253,30 @@ def box_room_depth(c2w, fx, fy, cx, cy, W, H, pillar=True, batch=16):
                 t = torch.where(hit, torch.minimum(t_in, t_wall), t_wall)
         out.append(t.to(torch.float32)[..., None])
     return torch.cat(out, 0)
+
+
+def box_room_color(c2w, fx, fy, cx, cy, W, H, batch=16):
+    """Colour images [B,H,W,3] float32 in [0.1, 0.9] of the BOX room (no pillar) seen from the c2w poses [B,4,4] (torch, any device):
+    each pixel's ray along K^-1 [j, i, 1] hits a wall, whose colour there is a smooth procedural texture of the hit point (a few
+    sinusoids per channel, periods 0.5 to 2 m), so that a trained render has a ground truth to converge to. Test and benchmark
+    infrastructure."""
+    import torch
+    dev = c2w.device
+    j = torch.arange(W, dtype=torch.float64, device=dev)
+    i = torch.arange(H, dtype=torch.float64, device=dev)
+    dc = torch.stack([((j[None, :] - cx) / fx).expand(H, W), ((i[:, None] - cy) / fy).expand(H, W), torch.ones(H, W, dtype=torch.float64,
+                                                                                                             device=dev)], -1)
+    box = torch.as_tensor(BOX, dtype=torch.float64, device=dev)
+    freq = torch.tensor([[3.1, 1.7, 4.3], [2.3, 5.1, 1.3], [4.7, 2.9, 3.7]], dtype=torch.float64, device=dev)
+    phase = torch.tensor([0.3, 1.9, 4.1], dtype=torch.float64, device=dev)
+    out = []
+    for b0 in range(0, c2w.shape[0], batch):
+        P = c2w[b0:b0 + batch].to(torch.float64)
+        o = P[:, None, None, :3, 3]
+        d = torch.einsum("brc,hwc->bhwr", P[:, :3, :3], dc)
+        with torch.no_grad():
+            t = torch.where(d > 0, (box - o) / d, torch.where(d < 0, (-box - o) / d, torch.full_like(d, float("inf")))).amin(-1)
+            x = o + t[..., None] * d
+            c = 0.5 + 0.2 * torch.sin(x @ freq.T + phase) + 0.2 * torch.sin(0.5 * (x @ freq) - phase)
+        out.append(c.clamp(0.1, 0.9).to(torch.float32))
+    return torch.cat(out, 0)

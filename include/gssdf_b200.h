@@ -714,6 +714,11 @@ typedef struct gssdf_adam_args {
     int32_t replay_only;     /* 1: row groups only, no gradient is read or written: every visited row is brought to `step` by replays */
 } gssdf_adam_args;
 int gssdf_adam_step(const gssdf_adam_args *a, gssdf_stream_t stream);
+/* gssdf_adam_step with one step count per group, as the reference's per-parameter Adam state keeps them when groups start stepping at
+   different iterations (gs_train's colour initialisation steps the SH groups alone): group_steps is a host array of n_groups steps >= 1
+   (a->step is ignored). The row groups must share one step, which replay->step equals and with which the visited rows are stamped.
+   Each group's update is gssdf_adam_step's at that step, bit for bit, in the same single launch. */
+int gssdf_adam_step_clocks(const gssdf_adam_args *a, const int32_t *group_steps, gssdf_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (e) data parallelism: sparse exchange of the splat gradient. Only the rows of the VISIBLE splats of a rank's frame carry a gradient
