@@ -50,9 +50,12 @@ static SsimWindow make_window() {  // loss_utils.cpp:6-14 (float tensor, normali
     return g;
 }
 
-// grid (strips / kSsimWarps, bands, C * 3); band_h rows per band
+// grid (strips / kSsimWarps, bands, C * 3); band_h rows per band. MASK: both images are multiplied by the image mask [H,W,3]
+// (nonzero = 1, shared by the C cameras) as they are loaded.
+template <bool MASK>
 __global__ void __launch_bounds__(kSsimWarps * 32)
-dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__restrict__ maps, const SsimSum red, int band_h) {
+dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__restrict__ maps, const SsimSum red, int band_h,
+                 const uint8_t *__restrict__ mask) {
     __shared__ float s_row[kSsimWarps][2][2][kRowW + 2];  // [warp][buffer][x | y][column]
     const int W = a.image_width, H = a.image_height;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -75,6 +78,11 @@ dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__r
         if (yy < 0 || yy >= H) return;
         if (ina) { xa = __ldg(X + ((int64_t)yy * W + ca) * 4); ya = __ldg(Y + ((int64_t)yy * W + ca) * 4); }
         if (inb) { xb = __ldg(X + ((int64_t)yy * W + cb) * 4); yb = __ldg(Y + ((int64_t)yy * W + cb) * 4); }
+        if (MASK) {
+            const float ma = ina && __ldg(mask + ((int64_t)yy * W + ca) * 3 + ch) ? 1.f : 0.f;
+            const float mb = inb && __ldg(mask + ((int64_t)yy * W + cb) * 3 + ch) ? 1.f : 0.f;
+            xa *= ma; ya *= ma; xb *= mb; yb *= mb;
+        }
     };
     float acc[kWin][5];
 #pragma unroll
@@ -142,8 +150,11 @@ dssim_fwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, float *__r
     }
 }
 
+// MASK: d/d rgb = m * d/d(rgb * m); for m in {0, 1} the masked pixels keep their cotangent, the others get the unmasked update (x * 1 = x)
+template <bool MASK>
 __global__ void __launch_bounds__(kSsimWarps * 32)
-dssim_bwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, const float *__restrict__ maps, float scale_grad, int band_h) {
+dssim_bwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, const float *__restrict__ maps, float scale_grad, int band_h,
+                 const uint8_t *__restrict__ mask) {
     __shared__ float s_row[kSsimWarps][2][3][kRowW + 2];  // [warp][buffer][map][column]
     const int W = a.image_width, H = a.image_height;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -175,10 +186,12 @@ dssim_bwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, const floa
     float *Vc = a.v_out_colors + (int64_t)cam * P * 4 + ch;
     // x, y and the cotangent of the output row completed by the NEXT row step are loaded one step ahead as well
     float xc = 0.f, yc = 0.f, vc = 0.f;
+    bool mc = true;
     auto fetch_out = [&](int py) {
         if (py >= y0 && py < y1 && px < W) {
             const int64_t pix = ((int64_t)py * W + px) * 4;
             xc = __ldg(Xc + pix); yc = __ldg(Yc + pix); vc = Vc[pix];
+            if (MASK) mc = __ldg(mask + ((int64_t)py * W + px) * 3 + ch) != 0;
         }
     };
     const int n_in = (y1 - y0) + 2 * kHalf;
@@ -210,7 +223,7 @@ dssim_bwd_kernel(const gssdf_dssim_loss_args a, const SsimWindow win, const floa
                 }
                 const int k_out = (j - (kWin - 1) + kWin) % kWin;
                 const int py = y0 + i - (kWin - 1);
-                if (i >= kWin - 1 && py < y1 && px < W) {  // one owner per (pixel, channel): plain read-modify-write, depth untouched
+                if (i >= kWin - 1 && py < y1 && px < W && (!MASK || mc)) {  // one owner per (pixel, channel): plain read-modify-write, depth untouched
                     Vc[((int64_t)py * W + px) * 4] = vc + scale_grad * (acc[k_out][0] + 2.f * xc * acc[k_out][1] + yc * acc[k_out][2]);
                 }
                 acc[k_out][0] = acc[k_out][1] = acc[k_out][2] = 0.f;
@@ -265,31 +278,48 @@ static int ssim_band_height(const void *kernel, int W, int H, int C) {
     return best;
 }
 
-extern "C" int gssdf_dssim_loss(const gssdf_dssim_loss_args *a, gssdf_stream_t stream) {
-    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "dssim_loss: null args");
-    GSSDF_REQUIRE(a->C > 0 && a->image_width > 0 && a->image_height > 0, GSSDF_EINVAL, "dssim_loss: bad image size");
-    GSSDF_REQUIRE(a->out_colors && a->gt && a->loss_out, GSSDF_EINVAL, "dssim_loss: null pointer");
+template <bool MASK>
+static int dssim_launch(const gssdf_dssim_loss_args *a, const uint8_t *mask, cudaStream_t st) {
     const DssimWs w = dssim_ws(a->C, a->image_width, a->image_height, a->workspace);
     GSSDF_REQUIRE(a->workspace && a->workspace_bytes >= w.bytes, GSSDF_ENOMEM, "dssim_loss: workspace too small");
     static const SsimWindow win = make_window();
     const double n = (double)a->C * 3.0 * a->image_width * a->image_height;
-    cudaStream_t st = (cudaStream_t)stream;
     const int gx = cdiv(cdiv(a->image_width, kStrip), kSsimWarps);
     {
-        const int band = ssim_band_height((const void *)dssim_fwd_kernel, a->image_width, a->image_height, a->C);
+        const int band = ssim_band_height((const void *)dssim_fwd_kernel<MASK>, a->image_width, a->image_height, a->C);
         const dim3 grid(gx, cdiv(a->image_height, band), a->C * 3);
         SsimSum red{reinterpret_cast<double *>(w.tail), reinterpret_cast<unsigned *>(w.tail + 8),
                     (unsigned)cdiv(a->image_width, kStrip) * grid.y * grid.z, (double)a->w_dssim / n};
         GSSDF_CUDA_OK(cudaMemsetAsync(w.tail, 0, 16, st));
-        dssim_fwd_kernel<<<grid, kSsimWarps * 32, 0, st>>>(*a, win, w.maps, red, band);
+        dssim_fwd_kernel<MASK><<<grid, kSsimWarps * 32, 0, st>>>(*a, win, w.maps, red, band, mask);
         GSSDF_LAUNCH_OK("dssim_fwd_kernel");
     }
     if (a->v_out_colors) {
-        const int band = ssim_band_height((const void *)dssim_bwd_kernel, a->image_width, a->image_height, a->C);
-        dssim_bwd_kernel<<<dim3(gx, cdiv(a->image_height, band), a->C * 3), kSsimWarps * 32, 0, st>>>(*a, win, w.maps, (float)(-a->w_dssim / n), band);
+        const int band = ssim_band_height((const void *)dssim_bwd_kernel<MASK>, a->image_width, a->image_height, a->C);
+        dssim_bwd_kernel<MASK><<<dim3(gx, cdiv(a->image_height, band), a->C * 3), kSsimWarps * 32, 0, st>>>(
+            *a, win, w.maps, (float)(-a->w_dssim / n), band, mask);
         GSSDF_LAUNCH_OK("dssim_bwd_kernel");
     }
     return GSSDF_OK;
+}
+
+static int check_dssim(const gssdf_dssim_loss_args *a) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "dssim_loss: null args");
+    GSSDF_REQUIRE(a->C > 0 && a->image_width > 0 && a->image_height > 0, GSSDF_EINVAL, "dssim_loss: bad image size");
+    GSSDF_REQUIRE(a->out_colors && a->gt && a->loss_out, GSSDF_EINVAL, "dssim_loss: null pointer");
+    return GSSDF_OK;
+}
+
+extern "C" int gssdf_dssim_loss(const gssdf_dssim_loss_args *a, gssdf_stream_t stream) {
+    if (int rc = check_dssim(a)) return rc;
+    return dssim_launch<false>(a, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int gssdf_dssim_loss_masked(const gssdf_dssim_loss_masked_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "dssim_loss_masked: null args");
+    if (int rc = check_dssim(&a->loss)) return rc;
+    GSSDF_REQUIRE(a->mask != nullptr, GSSDF_EINVAL, "dssim_loss_masked: null mask");
+    return dssim_launch<true>(&a->loss, a->mask, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------

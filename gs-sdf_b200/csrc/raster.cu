@@ -601,7 +601,10 @@ __device__ __forceinline__ void cam_rot(const float *viewmats, int cam, float R[
         for (int c = 0; c < 3; ++c) R[r * 3 + c] = v[r * 4 + c];
 }
 
-__global__ void __launch_bounds__(256) render_post_fwd_kernel(const gssdf_render_post_fwd_args a) {
+// BG: the background composited into the colour (gssdf_render_post_bg_fwd): 0 none (black), 1 white, 2 the per-pixel image bg.
+// Each step is rounded on its own, as ATen evaluates c + (1 - alpha) * bg: an FMA would not give the reference's bits.
+template <int BG>
+__global__ void __launch_bounds__(256) render_post_fwd_kernel(const gssdf_render_post_fwd_args a, const float *__restrict__ bg) {
     const int64_t P = (int64_t)a.image_width * a.image_height;
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= P * a.C) return;
@@ -613,15 +616,27 @@ __global__ void __launch_bounds__(256) render_post_fwd_kernel(const gssdf_render
     float ed = d / al;
     if (isnan(ed)) ed = 0.f;
     else if (isinf(ed)) ed = ed > 0 ? 3.402823466e38f : -3.402823466e38f;
-    reinterpret_cast<float4 *>(a.out_colors)[p] =
-        make_float4(a.render_colors[3 * p], a.render_colors[3 * p + 1], a.render_colors[3 * p + 2], ed);
+    float c0 = a.render_colors[3 * p], c1 = a.render_colors[3 * p + 1], c2 = a.render_colors[3 * p + 2];
+    if (BG != 0) {
+        const float t = __fsub_rn(1.f, al);
+        if (BG == 1) {
+            c0 = __fadd_rn(c0, t); c1 = __fadd_rn(c1, t); c2 = __fadd_rn(c2, t);
+        } else {
+            c0 = __fadd_rn(c0, __fmul_rn(t, bg[3 * p]));
+            c1 = __fadd_rn(c1, __fmul_rn(t, bg[3 * p + 1]));
+            c2 = __fadd_rn(c2, __fmul_rn(t, bg[3 * p + 2]));
+        }
+    }
+    reinterpret_cast<float4 *>(a.out_colors)[p] = make_float4(c0, c1, c2, ed);
     // n_world = n_cam * inverse(V)[:3,:3]^T = n_cam * R  (R_c2w^T == R for a rigid world->camera V)
     const float n0 = a.render_normals[3 * p], n1 = a.render_normals[3 * p + 1], n2 = a.render_normals[3 * p + 2];
 #pragma unroll
     for (int c = 0; c < 3; ++c) a.out_normals[3 * p + c] = n0 * R[c] + n1 * R[3 + c] + n2 * R[6 + c];
 }
 
-__global__ void __launch_bounds__(256) render_post_bwd_kernel(const gssdf_render_post_bwd_args a) {
+// the background's alpha cotangent: d/d alpha of c + (1 - alpha) * bg is -bg per channel
+template <int BG>
+__global__ void __launch_bounds__(256) render_post_bwd_kernel(const gssdf_render_post_bwd_args a, const float *__restrict__ bg) {
     const int64_t P = (int64_t)a.image_width * a.image_height;
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= P * a.C) return;
@@ -637,6 +652,8 @@ __global__ void __launch_bounds__(256) render_post_bwd_kernel(const gssdf_render
         vdep = vo.w / al;
         val += -vo.w * d / (al * al);
     }
+    if (BG == 1) val += -(vo.x + vo.y + vo.z);
+    if (BG == 2) val += -(vo.x * bg[3 * p] + vo.y * bg[3 * p + 1] + vo.z * bg[3 * p + 2]);
     a.v_render_depths[p] = vdep;
     a.v_render_alphas[p] = val;
     const float g0 = a.v_out_normals[3 * p], g1 = a.v_out_normals[3 * p + 1], g2 = a.v_out_normals[3 * p + 2];
@@ -644,15 +661,22 @@ __global__ void __launch_bounds__(256) render_post_bwd_kernel(const gssdf_render
     for (int r = 0; r < 3; ++r) a.v_render_normals[3 * p + r] = g0 * R[r * 3] + g1 * R[r * 3 + 1] + g2 * R[r * 3 + 2];
 }
 
-// f-1 (minimal): L1 photometric + depth loss and its cotangent in one pass
-__global__ void __launch_bounds__(256) l1_loss_kernel(const gssdf_l1_loss_args a, int64_t n_pix) {
+// f-1 (minimal): L1 photometric + depth loss and its cotangent in one pass. MASK: the rgb differences are multiplied by the image
+// mask [H,W,3] (nonzero = 1) shared by the C cameras; the depth term is not masked and the mean keeps its denominator.
+template <bool MASK>
+__global__ void __launch_bounds__(256) l1_loss_kernel(const gssdf_l1_loss_args a, int64_t n_pix, const uint8_t *__restrict__ mask) {
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     float part = 0.f;
     if (p < n_pix) {
         const float4 o = reinterpret_cast<const float4 *>(a.out_colors)[p];
         const float4 g = reinterpret_cast<const float4 *>(a.gt)[p];
         const float sr = a.w_rgb / (3.f * (float)n_pix), sd = a.w_depth / (float)n_pix;
-        const float d0 = o.x - g.x, d1 = o.y - g.y, d2 = o.z - g.z, d3 = o.w - g.w;
+        float d0 = o.x - g.x, d1 = o.y - g.y, d2 = o.z - g.z;
+        const float d3 = o.w - g.w;
+        if (MASK) {
+            const uint8_t *m = mask + 3 * (p % ((int64_t)a.image_width * a.image_height));
+            d0 *= m[0] ? 1.f : 0.f; d1 *= m[1] ? 1.f : 0.f; d2 *= m[2] ? 1.f : 0.f;  // sgn(d * m) * m == sgn(d * m) for m in {0, 1}
+        }
         part = sr * (fabsf(d0) + fabsf(d1) + fabsf(d2)) + sd * fabsf(d3);
         auto sgn = [](float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); };
         reinterpret_cast<float4 *>(a.v_out_colors)[p] = make_float4(sr * sgn(d0), sr * sgn(d1), sr * sgn(d2), sd * sgn(d3));
@@ -672,12 +696,27 @@ __global__ void __launch_bounds__(256) l1_loss_kernel(const gssdf_l1_loss_args a
 
 using namespace gssdf;
 
-extern "C" int gssdf_l1_loss(const gssdf_l1_loss_args *a, gssdf_stream_t stream) {
+static int check_l1(const gssdf_l1_loss_args *a) {
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "l1_loss: null args");
     GSSDF_REQUIRE(a->C > 0 && a->image_width > 0 && a->image_height > 0, GSSDF_EINVAL, "l1_loss: bad image size");
     GSSDF_REQUIRE(a->out_colors && a->gt && a->loss_out && a->v_out_colors, GSSDF_EINVAL, "l1_loss: null pointer");
+    return GSSDF_OK;
+}
+
+extern "C" int gssdf_l1_loss(const gssdf_l1_loss_args *a, gssdf_stream_t stream) {
+    if (int rc = check_l1(a)) return rc;
     const int64_t n = (int64_t)a->C * a->image_width * a->image_height;
-    l1_loss_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(*a, n);
+    l1_loss_kernel<false><<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(*a, n, nullptr);
+    GSSDF_LAUNCH_OK("l1_loss_kernel");
+    return GSSDF_OK;
+}
+
+extern "C" int gssdf_l1_loss_masked(const gssdf_l1_loss_masked_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "l1_loss_masked: null args");
+    if (int rc = check_l1(&a->loss)) return rc;
+    GSSDF_REQUIRE(a->mask != nullptr, GSSDF_EINVAL, "l1_loss_masked: null mask");
+    const int64_t n = (int64_t)a->loss.C * a->loss.image_width * a->loss.image_height;
+    l1_loss_kernel<true><<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(a->loss, n, a->mask);
     GSSDF_LAUNCH_OK("l1_loss_kernel");
     return GSSDF_OK;
 }
@@ -820,26 +859,72 @@ extern "C" int gssdf_raster2dgs_bwd(const gssdf_raster2dgs_bwd_args *a, gssdf_st
     return GSSDF_OK;
 }
 
-extern "C" int gssdf_render_post_fwd(const gssdf_render_post_fwd_args *a, gssdf_stream_t stream) {
+static int check_post_fwd(const gssdf_render_post_fwd_args *a) {
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "render_post_fwd: null args");
     GSSDF_REQUIRE(a->C > 0 && a->image_width > 0 && a->image_height > 0, GSSDF_EINVAL, "render_post_fwd: bad image size");
     GSSDF_REQUIRE(a->viewmats && a->render_colors && a->render_depths && a->render_alphas && a->render_normals && a->out_colors &&
                       a->out_normals,
                   GSSDF_EINVAL, "render_post_fwd: null pointer");
-    const int64_t n = (int64_t)a->C * a->image_width * a->image_height;
-    render_post_fwd_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(*a);
-    GSSDF_LAUNCH_OK("render_post_fwd_kernel");
     return GSSDF_OK;
 }
 
-extern "C" int gssdf_render_post_bwd(const gssdf_render_post_bwd_args *a, gssdf_stream_t stream) {
+static int check_post_bwd(const gssdf_render_post_bwd_args *a) {
     GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "render_post_bwd: null args");
     GSSDF_REQUIRE(a->C > 0 && a->image_width > 0 && a->image_height > 0, GSSDF_EINVAL, "render_post_bwd: bad image size");
     GSSDF_REQUIRE(a->viewmats && a->render_depths && a->render_alphas && a->v_out_colors && a->v_out_normals && a->v_render_colors &&
                       a->v_render_depths && a->v_render_alphas && a->v_render_normals,
                   GSSDF_EINVAL, "render_post_bwd: null pointer");
-    const int64_t n = (int64_t)a->C * a->image_width * a->image_height;
-    render_post_bwd_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(*a);
+    return GSSDF_OK;
+}
+
+static int check_bg(const char *who, int32_t mode, const float *bg) {
+    GSSDF_REQUIRE(mode >= 0 && mode <= 2, GSSDF_EINVAL, "%s: bck_mode %d is not 0, 1 or 2", who, mode);
+    GSSDF_REQUIRE(mode != 2 || bg != nullptr, GSSDF_EINVAL, "%s: bck_mode 2 needs a background image", who);
+    return GSSDF_OK;
+}
+
+template <int BG>
+static int launch_post_fwd(const gssdf_render_post_fwd_args &a, const float *bg, cudaStream_t st) {
+    const int64_t n = (int64_t)a.C * a.image_width * a.image_height;
+    render_post_fwd_kernel<BG><<<cdiv(n, 256), 256, 0, st>>>(a, bg);
+    GSSDF_LAUNCH_OK("render_post_fwd_kernel");
+    return GSSDF_OK;
+}
+
+template <int BG>
+static int launch_post_bwd(const gssdf_render_post_bwd_args &a, const float *bg, cudaStream_t st) {
+    const int64_t n = (int64_t)a.C * a.image_width * a.image_height;
+    render_post_bwd_kernel<BG><<<cdiv(n, 256), 256, 0, st>>>(a, bg);
     GSSDF_LAUNCH_OK("render_post_bwd_kernel");
     return GSSDF_OK;
+}
+
+extern "C" int gssdf_render_post_fwd(const gssdf_render_post_fwd_args *a, gssdf_stream_t stream) {
+    if (int rc = check_post_fwd(a)) return rc;
+    return launch_post_fwd<0>(*a, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int gssdf_render_post_bwd(const gssdf_render_post_bwd_args *a, gssdf_stream_t stream) {
+    if (int rc = check_post_bwd(a)) return rc;
+    return launch_post_bwd<0>(*a, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int gssdf_render_post_bg_fwd(const gssdf_render_post_bg_fwd_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "render_post_bg_fwd: null args");
+    if (int rc = check_post_fwd(&a->post)) return rc;
+    if (int rc = check_bg("render_post_bg_fwd", a->bck_mode, a->bg)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (a->bck_mode == 1) return launch_post_fwd<1>(a->post, nullptr, st);
+    if (a->bck_mode == 2) return launch_post_fwd<2>(a->post, a->bg, st);
+    return launch_post_fwd<0>(a->post, nullptr, st);
+}
+
+extern "C" int gssdf_render_post_bg_bwd(const gssdf_render_post_bg_bwd_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "render_post_bg_bwd: null args");
+    if (int rc = check_post_bwd(&a->post)) return rc;
+    if (int rc = check_bg("render_post_bg_bwd", a->bck_mode, a->bg)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (a->bck_mode == 1) return launch_post_bwd<1>(a->post, nullptr, st);
+    if (a->bck_mode == 2) return launch_post_bwd<2>(a->post, a->bg, st);
+    return launch_post_bwd<0>(a->post, nullptr, st);
 }

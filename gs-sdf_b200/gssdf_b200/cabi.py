@@ -187,6 +187,34 @@ def l1_loss(Cn, W, H, out_colors, gt, w_rgb, w_depth, loss_out, v_out_colors):
     check(lib().gssdf_l1_loss(_lib.C.byref(a), _stream()))
 
 
+def render_post_bg_fwd(Cn, W, H, viewmats, render_colors, render_depths, render_alphas, render_normals, out_colors, out_normals,
+                       bck_mode, bg=None):
+    """render_post_fwd with the background composited into the colour: bck_mode 0 black, 1 white, 2 bg [C,H,W,3]."""
+    post = make_args("gssdf_render_post_fwd_args", C=Cn, image_width=W, image_height=H, viewmats=viewmats,
+                     render_colors=render_colors, render_depths=render_depths, render_alphas=render_alphas,
+                     render_normals=render_normals, out_colors=out_colors, out_normals=out_normals)
+    a = make_args("gssdf_render_post_bg_fwd_args", post=post, bck_mode=int(bck_mode), bg=bg)
+    check(lib().gssdf_render_post_bg_fwd(_lib.C.byref(a), _stream()))
+
+
+def render_post_bg_bwd(Cn, W, H, viewmats, render_depths, render_alphas, v_out_colors, v_out_normals, v_alphas_in,
+                       v_render_colors, v_render_depths, v_render_alphas, v_render_normals, bck_mode, bg=None):
+    post = make_args("gssdf_render_post_bwd_args", C=Cn, image_width=W, image_height=H, viewmats=viewmats,
+                     render_depths=render_depths, render_alphas=render_alphas, v_out_colors=v_out_colors,
+                     v_out_normals=v_out_normals, v_alphas_in=v_alphas_in, v_render_colors=v_render_colors,
+                     v_render_depths=v_render_depths, v_render_alphas=v_render_alphas, v_render_normals=v_render_normals)
+    a = make_args("gssdf_render_post_bg_bwd_args", post=post, bck_mode=int(bck_mode), bg=bg)
+    check(lib().gssdf_render_post_bg_bwd(_lib.C.byref(a), _stream()))
+
+
+def l1_loss_masked(Cn, W, H, out_colors, gt, w_rgb, w_depth, loss_out, v_out_colors, mask):
+    """l1_loss with the rgb differences multiplied by mask (uint8 [H,W,3], nonzero = 1, shared by the C cameras)."""
+    loss = make_args("gssdf_l1_loss_args", C=Cn, image_width=W, image_height=H, out_colors=out_colors, gt=gt, w_rgb=w_rgb,
+                     w_depth=w_depth, loss_out=loss_out, v_out_colors=v_out_colors)
+    a = make_args("gssdf_l1_loss_masked_args", loss=loss, mask=mask)
+    check(lib().gssdf_l1_loss_masked(_lib.C.byref(a), _stream()))
+
+
 # ---- SDF branch -------------------------------------------------------------------------------
 def sdf_net(table_half, mlp, n_levels=16, n_features=2, log2_hashmap_size=19, base_resolution=32, per_level_scale=2.0,
             hidden_dim=64, n_hidden=3, origin=(0.0, 0.0, 0.0), inv_size=0.0, mlp_mode=0, mlp_packed=None):
@@ -263,6 +291,16 @@ def dssim_loss(Cn, W, H, out_colors, gt, w_dssim, loss_out, v_out_colors, ws):
     a = make_args("gssdf_dssim_loss_args", C=Cn, image_width=W, image_height=H, out_colors=out_colors, gt=gt, w_dssim=w_dssim,
                   loss_out=loss_out, v_out_colors=v_out_colors, workspace=w, workspace_bytes=w.numel())
     check(lib().gssdf_dssim_loss(_lib.C.byref(a), _stream()))
+
+
+def dssim_loss_masked(Cn, W, H, out_colors, gt, w_dssim, loss_out, v_out_colors, ws, mask):
+    """dssim_loss of rgb * mask against gt * mask (mask uint8 [H,W,3], nonzero = 1); the gradient is masked too."""
+    need = lib().gssdf_dssim_workspace_bytes(Cn, W, H)
+    w = ws.get(need)
+    loss = make_args("gssdf_dssim_loss_args", C=Cn, image_width=W, image_height=H, out_colors=out_colors, gt=gt, w_dssim=w_dssim,
+                     loss_out=loss_out, v_out_colors=v_out_colors, workspace=w, workspace_bytes=w.numel())
+    a = make_args("gssdf_dssim_loss_masked_args", loss=loss, mask=mask)
+    check(lib().gssdf_dssim_loss_masked(_lib.C.byref(a), _stream()))
 
 
 # ---- operator-level hash grid (tcnn_binding twin), gate, optimiser, remaining loss terms ------------------------------------

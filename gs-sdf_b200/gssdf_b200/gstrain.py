@@ -76,15 +76,23 @@ class GsTrainer:
     poses: [T,4,4] camera-to-world (OpenCV axes); K: [3,3] pinhole; images: float32 [T,H,W,3] in [0,1], on the device or in pinned host
         memory (then one frame is copied per iteration, asynchronously).
     spatial_scale: 0.5 * inner_map_size. The remaining keywords are config/base.yaml's keys with its defaults; `densify` holds Densifier's
-    keywords (prune_opa .. sh_degree_interval; sh_degree and sh_degree_interval are passed through from here)."""
+    keywords (prune_opa .. sh_degree_interval; sh_degree and sh_degree_interval are passed through from here).
+    bck_color: the scene's k_bck_color, the background every render composites (colour initialisation, joint iterations, render()):
+        0 black, 1 white (FAST-LIVO2, Oxford Spires, HKU), 2 a uniform random image drawn before every render from a device generator of
+        its own (`bg_gen`, seeded from `seed`; the splat samples' draws stay those of modes 0 and 1).
+    mask: the dataset's image mask, bool or uint8 [H,W], [H,W,1] or [H,W,3] on the device (nonzero = keep), applied to every frame's L1
+        and DSSIM terms as loss::rgb_loss / dssim_loss do."""
 
     def __init__(self, sdf, splats, poses, K, images, *, capacity, spatial_scale, gs_iter_step=30000, color_init=True,
                  detach_sdf_grad=False, refine_gs_struct_start_iter=3000, rgb_weight=0.8, dssim_weight=0.2, render_normal_weight=0.01,
                  isotropic_weight=0.05, gs_sdf_weight=1e-3, visible_thr=0.1, outlier_remove=False, outlier_dist=0.05,
-                 outlier_removal_interval=2000, sh_degree=3, sh_degree_interval=1000, densify=None, isect_cap=None, seed=0):
+                 outlier_removal_interval=2000, sh_degree=3, sh_degree_interval=1000, densify=None, isect_cap=None, seed=0, bck_color=0,
+                 mask=None):
         dev = sdf.dev
         if not (gs_iter_step >= 1 and outlier_removal_interval >= 1 and sh_degree_interval >= 1):
             raise ValueError("GsTrainer: gs_iter_step, outlier_removal_interval and sh_degree_interval must be >= 1")
+        hw = tuple(images.shape[1:3]) if isinstance(images, torch.Tensor) and images.dim() == 4 else (None, None)
+        RD.check_photometric("GsTrainer", bck_color, mask, hw[0], hw[1], dev)
         for k in ("xyz", "origin", "direction", "depth"):
             if not sdf.pack[k].is_cuda:
                 raise ValueError(f"GsTrainer: the SdfTrainer's pack[{k!r}] must be on the device")
@@ -115,7 +123,7 @@ class GsTrainer:
                                      sh_degree=sh_degree, bce_sigma=sdf.bce_sigma, eikonal_weight=sdf.eik_w, gs_sdf_weight=gs_sdf_weight,
                                      visible_thr=visible_thr, mlp_mode=1, eikonal_mode=1, align_weight=sdf.align_w, rgb_weight=rgb_weight,
                                      dssim_weight=dssim_weight, depth_weight=0.0, normal_weight=0.0, isotropic_weight=isotropic_weight,
-                                     spatial_scale=self.spatial_scale, n_live=n0, delta_dev=sdf.std_dev)
+                                     spatial_scale=self.spatial_scale, n_live=n0, delta_dev=sdf.std_dev, bck_color=bck_color, mask=mask)
         T.origin, T.inv_size, T.bce_isigma = net.origin, net.inv_size, sdf.bce_isigma
         T.set_octree(sdf.rs.tree)
         n_sdf = sdf.n_table + sdf.n_mlp
@@ -131,6 +139,7 @@ class GsTrainer:
         self.sdf_steps0 = sdf.t
         self.cpu_gen = torch.Generator().manual_seed(seed)
         self.gen = torch.Generator(dev).manual_seed(seed)
+        self.bg_gen = torch.Generator(dev).manual_seed(seed + (1 << 32))  # bck_color 2's backgrounds: not the randns stream
         self.randns = torch.empty(T.R.cap, 2, dtype=torch.float32, device=dev)  # the splat samples' draw, fresh every render
         self.perm = None
         self.gt = torch.zeros(1, H, W, 4, dtype=torch.float32, device=dev)  # RGB + the (unused) depth channel the loss kernels read
@@ -159,6 +168,11 @@ class GsTrainer:
             self.gt[0, ..., :3].copy_(self.stage)
         return self.viewmats[cam:cam + 1]
 
+    def draw_background(self):
+        """bck_color 2: a fresh uniform background for the next render (torch::rand({H,W,3}), neural_gaussian.cpp:545-547)."""
+        if self.T.bg is not None:
+            self.T.bg.uniform_(generator=self.bg_gen)
+
     def run_color_init(self):
         """gs_train's color_init block (:364-387): train_num iterations of gs_train_batch_iter(i, false) + Adam over the SH groups."""
         T = self.T
@@ -167,6 +181,7 @@ class GsTrainer:
         T.set_live(T.N_live)
         for i in range(self.train_num):
             vm = self.load_frame(self.camera(i))
+            self.draw_background()
             T.color_step(vm, self.Ks, self.gt)
             self.h_color[i:i + 1].copy_(T.R.loss)
         T.lr = [color_init_lr(lr) for lr in base]
@@ -186,6 +201,7 @@ class GsTrainer:
         vm = self.load_frame(self.camera(i))
         T.normal_w = self.normal_w if normal_on(i, self.refine_struct_start) else 0.0
         self.randns.normal_(generator=self.gen)  # the reference's randn of every render (Projection.cpp:728)
+        self.draw_background()
         if self.detach:
             loss, sdf_loss = T.train_step(vm, self.Ks, self.gt, None, None, self.randns)
         else:
@@ -249,13 +265,15 @@ class GsTrainer:
         return dict(net=self.sdf.net_mod, splats=splats, render=self.render)
 
     def render(self, viewmat):
-        """The colour image [H,W,3] of a world->camera pose [4,4] at the current SH degree (the render the reference exports and scores)."""
+        """The colour image [H,W,3] of a world->camera pose [4,4] at the current SH degree on the configured background (the render the
+        reference exports and scores; bck_color 2 draws a fresh background for it)."""
         T = self.T
         T.flush_sh()
         vm = torch.as_tensor(viewmat, dtype=torch.float32).reshape(1, 4, 4).to(self.dev).contiguous()
         sc = T.scene
         raw = dict(sc["raw"], sh_catch_up=None)
-        T.R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], vm, self.Ks, raw=raw)
+        self.draw_background()
+        T.R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], vm, self.Ks, raw=raw, bck_color=T.bck_color, bg=T.bg)
         return T.R.out_colors[0, ..., :3].clone()
 
     def __repr__(self):

@@ -16,6 +16,27 @@ import torch
 from . import cabi
 
 
+def check_photometric(who, bck_color, mask, H, W, device):
+    """The background mode and image mask of the photometric path (DESIGN 7o), checked before any device work: bck_color 0 (black),
+    1 (white) or 2 (random); mask None or a bool / uint8 tensor [H,W], [H,W,1] or [H,W,3] on the CUDA device `device`."""
+    if isinstance(bck_color, bool) or bck_color not in (0, 1, 2):
+        raise ValueError(f"{who}: bck_color must be 0 (black), 1 (white) or 2 (random), got {bck_color!r}")
+    if mask is None:
+        return
+    if not isinstance(mask, torch.Tensor) or mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"{who}: mask must be a bool or uint8 tensor, got {getattr(mask, 'dtype', type(mask))}")
+    if H is not None and tuple(mask.shape) not in ((H, W), (H, W, 1), (H, W, 3)):
+        raise ValueError(f"{who}: mask must be [H,W], [H,W,1] or [H,W,3] with H={H}, W={W}, got {tuple(mask.shape)}")
+    dev = torch.device(device)
+    if not mask.is_cuda or dev.type != "cuda" or (dev.index is not None and mask.device.index != dev.index):
+        raise ValueError(f"{who}: mask must be on {dev}, got {mask.device}")
+
+
+def expand_mask(mask, H, W):
+    """A checked mask as the masked loss kernels read it: uint8 [H,W,3], nonzero -> 1 (the reference's bool mask)."""
+    return None if mask is None else mask.reshape(H, W, -1).ne(0).to(torch.uint8).expand(H, W, 3).contiguous()
+
+
 class SplatRenderer:
     def __init__(self, N, K, C, W, H, device, isect_cap, tile_size=16, near=0.05, far=300.0, sh_degree=3, presort_cull=True):
         self.N, self.K, self.C, self.W, self.H, self.tile = N, K, C, W, H, tile_size
@@ -73,9 +94,11 @@ class SplatRenderer:
             self.stage_events.append((name, ev))
 
     # -- forward ------------------------------------------------------------------------------
-    def forward(self, means, quats, scales, opacities, sh, viewmats, Ks, randns=None, raw=None):
+    def forward(self, means, quats, scales, opacities, sh, viewmats, Ks, randns=None, raw=None, bck_color=0, bg=None):
         """raw = dict(offsets=[N,3], sh_rest=[N,K-1,3]) switches to the RAW parameters of NeuralGS (row a1 fused into the kernels):
-        means = anchors, scales = log-scales, opacities = logits, sh = features_dc; no activated copies are materialised."""
+        means = anchors, scales = log-scales, opacities = logits, sh = features_dc; no activated copies are materialised.
+        bck_color: the background composited into out_colors after the rasteriser (NeuralGS::render): 0 black, 1 white, 2 the image
+        bg [C,H,W,3]."""
         C, W, H, cap = self.C, self.W, self.H, self.cap
         off, rest = (raw["offsets"], raw["sh_rest"]) if raw else (None, None)
         cabi.project2dgs_fwd(means, quats, scales, viewmats, Ks, W, H, self.near, self.far, 0.0, randns, cap, self.p,
@@ -97,17 +120,23 @@ class SplatRenderer:
                             self.p["pt_opacities"], self.p["normals"], None, self.offsets, self.flatten_ids, self.r, self.raster_ws,
                             prof=self.prof_fwd, isect_cap=self.isect_cap)
         self._mark("raster_fwd")
-        cabi.render_post_fwd(C, W, H, viewmats, self.r["render_colors"], self.r["render_depths"], self.r["render_alphas"],
-                             self.r["render_normals"], self.out_colors, self.out_normals)
+        if bck_color:
+            cabi.render_post_bg_fwd(C, W, H, viewmats, self.r["render_colors"], self.r["render_depths"], self.r["render_alphas"],
+                                    self.r["render_normals"], self.out_colors, self.out_normals, bck_color, bg)
+        else:
+            cabi.render_post_fwd(C, W, H, viewmats, self.r["render_colors"], self.r["render_depths"], self.r["render_alphas"],
+                                 self.r["render_normals"], self.out_colors, self.out_normals)
         self._mark("post_fwd")
         return self.out_colors, self.out_normals
 
     # -- loss + backward -----------------------------------------------------------------------
     def backward(self, means, quats, scales, opacities, sh, viewmats, Ks, gt, randns=None, w_rgb=1.0, w_depth=0.1, v_samples=None,
-                 zero_grads=True, raw=None, w_dssim=0.0, w_normal=0.0, w_isotropic=0.0, before_projection_bwd=None, projection_bwd=True):
+                 zero_grads=True, raw=None, w_dssim=0.0, w_normal=0.0, w_isotropic=0.0, before_projection_bwd=None, projection_bwd=True,
+                 bck_color=0, bg=None, mask=None):
         """With raw parameters the flat gradient holds dL/d(offsets|quats|log-scales|logits|features_dc|features_rest); the SH segment
         keeps its [N,K,3] size, laid out as dc [N,1,3] followed by rest [N,K-1,3]. projection_bwd=False stops after the SH backward (the
-        structure is frozen: only the colour gradient is wanted)."""
+        structure is frozen: only the colour gradient is wanted). bck_color / bg: those of the forward; mask: uint8 [H,W,3]
+        (expand_mask) multiplying both images in the L1 and DSSIM terms (loss::rgb_loss / dssim_loss with a mask)."""
         C, W, H, cap = self.C, self.W, self.H, self.cap
         off, rest = (raw["offsets"], raw["sh_rest"]) if raw else (None, None)
         N, K = self.N, self.K
@@ -116,9 +145,15 @@ class SplatRenderer:
         self.loss.zero_()
         if zero_grads:
             self.flat_grad.zero_()
-        cabi.l1_loss(C, W, H, self.out_colors, gt, w_rgb, w_depth, self.loss, self.v_out_colors)
+        if mask is None:
+            cabi.l1_loss(C, W, H, self.out_colors, gt, w_rgb, w_depth, self.loss, self.v_out_colors)
+        else:
+            cabi.l1_loss_masked(C, W, H, self.out_colors, gt, w_rgb, w_depth, self.loss, self.v_out_colors, mask)
         if w_dssim > 0:  # + w_dssim * (1 - SSIM(rgb, gt)) (loss::dssim_loss), gradient added to the colour cotangent
-            cabi.dssim_loss(C, W, H, self.out_colors, gt, w_dssim, self.loss, self.v_out_colors, self.loss_ws)
+            if mask is None:
+                cabi.dssim_loss(C, W, H, self.out_colors, gt, w_dssim, self.loss, self.v_out_colors, self.loss_ws)
+            else:
+                cabi.dssim_loss_masked(C, W, H, self.out_colors, gt, w_dssim, self.loss, self.v_out_colors, self.loss_ws, mask)
         if w_normal > 0:  # normal consistency between the rendered normals and the normals of the expected-depth map
                           # (neural_mapping.cpp:243-266): adds to the ED cotangent (channel 3) and overwrites the normal cotangent
             cabi.normal_consistency_loss(C, W, H, viewmats, Ks, self.out_colors.data_ptr() + 12, 4, self.r["render_alphas"], self.out_normals,
@@ -131,9 +166,14 @@ class SplatRenderer:
         if w_isotropic > 0:  # isotropic regulariser on the visible splats' (x, y) scales (neural_mapping.cpp:268-276)
             cabi.isotropic_loss(self.N, cap, self.counts, self.p["gaussian_ids"], scales, raw is not None, w_isotropic, self.loss,
                                 self.v_scales)
-        cabi.render_post_bwd(C, W, H, viewmats, self.r["render_depths"], self.r["render_alphas"], self.v_out_colors,
-                             self.v_out_normals, None, self.v_r["colors"], self.v_r["depths"], self.v_r["alphas"],
-                             self.v_r["normals"])
+        if bck_color:
+            cabi.render_post_bg_bwd(C, W, H, viewmats, self.r["render_depths"], self.r["render_alphas"], self.v_out_colors,
+                                    self.v_out_normals, None, self.v_r["colors"], self.v_r["depths"], self.v_r["alphas"],
+                                    self.v_r["normals"], bck_color, bg)
+        else:
+            cabi.render_post_bwd(C, W, H, viewmats, self.r["render_depths"], self.r["render_alphas"], self.v_out_colors,
+                                 self.v_out_normals, None, self.v_r["colors"], self.v_r["depths"], self.v_r["alphas"],
+                                 self.v_r["normals"])
         self._mark("losses+post_bwd")
         cabi.raster2dgs_bwd(C, W, H, self.tile, 3, cap, self.counts, self.p["means2d"], self.p["ray_transforms"], self.colors,
                             self.p["pt_opacities"], self.p["normals"], None, self.offsets, self.flatten_ids,
@@ -189,10 +229,16 @@ class GsSdfStep:
     def __init__(self, N, K, W, H, device, isect_cap, sdf_net_cfg, n_ray_samples=32768, sh_degree=3, origin=(0.0, 0.0, 0.0),
                  map_size=14.0, bce_sigma=0.1, delta=None, eikonal_weight=0.1, gs_sdf_weight=1e-3, visible_thr=0.1, mlp_mode=None,
                  eikonal_mode=None, align_weight=0.1, rgb_weight=0.8, dssim_weight=0.2, depth_weight=0.1, normal_weight=0.0,
-                 isotropic_weight=0.0, delta_dev=None):
+                 isotropic_weight=0.0, delta_dev=None, bck_color=0, mask=None):
         """delta_dev: float32 CUDA tensor [1] read by every SDF call of [A] and [C] in place of the host scalar `delta` (the sample std the
-        SDF stage adapts on the device, nsdf.SdfTrainer.std_dev); the ray-site forward then also evaluates the base variant into ray_y1."""
+        SDF stage adapts on the device, nsdf.SdfTrainer.std_dev); the ray-site forward then also evaluates the base variant into ray_y1.
+        bck_color (k_bck_color: 0 black, 1 white, 2 random) and mask (bool / uint8 [H,W], [H,W,1] or [H,W,3] on the device, one for every
+        frame): the render's background and the photometric loss's image mask (DESIGN 7o), in the joint step and in color_step. With
+        bck_color 2 the render composites self.bg [1,H,W,3], which the caller fills before every render (gstrain.GsTrainer draws it)."""
+        check_photometric("GsSdfStep", bck_color, mask, H, W, device)
         self.R = SplatRenderer(N, K, 1, W, H, device, isect_cap, sh_degree=sh_degree)
+        self.bck_color, self.mask = int(bck_color), expand_mask(mask, H, W)
+        self.bg = torch.zeros(1, H, W, 3, dtype=torch.float32, device=device) if self.bck_color == 2 else None
         self.dev, self.N, self.n_ray = device, N, n_ray_samples
         self.cfg = dict(sdf_net_cfg)
         self.origin, self.inv_size = tuple(origin), 1.0 / map_size
@@ -377,7 +423,7 @@ class GsSdfStep:
             self.flat_grad[:t0].zero_()
         # [B] render
         R.forward(scene["means"], scene["quats"], scene["scales"], scene["opacities"], scene["sh"], viewmats, Ks, randns,
-                  raw=scene.get("raw"))
+                  raw=scene.get("raw"), bck_color=self.bck_color, bg=self.bg)
         # [C] coupling on the stochastic splat samples (rows < nnz, counted on the device)
         samples, n_live = R.p["samples"], R.counts  # counts[0] == nnz
         # the reference's sample gate: vis > visible_thr (& octree validity), counted on the device (no nonzero() / .item() sync)
@@ -399,7 +445,8 @@ class GsSdfStep:
             wait_c = (lambda: torch.cuda.current_stream().wait_event(self._ev_c)) if side is not None else None
             loss = R.backward(scene["means"], scene["quats"], scene["scales"], scene["opacities"], scene["sh"], viewmats, Ks, gt_image, randns,
                               v_samples=self.v_samples, zero_grads=False, raw=scene.get("raw"), w_rgb=self.rgb_w, w_depth=self.depth_w,
-                              w_dssim=self.dssim_w, w_normal=self.normal_w, w_isotropic=self.iso_w, before_projection_bwd=wait_c)
+                              w_dssim=self.dssim_w, w_normal=self.normal_w, w_isotropic=self.iso_w, before_projection_bwd=wait_c,
+                              bck_color=self.bck_color, bg=self.bg, mask=self.mask)
             return loss, self.sdf_loss
         cabi.sdf_gate_count(cap, self.n_gate, visibilities=R.r["visibilities"], visible_thr=self.vis_thr, valid_mask=self.valid_mask,
                             n_live=n_live)
@@ -436,7 +483,8 @@ class GsSdfStep:
         # [D] photometric loss + backward of the render, with the coupling gradient entering through the samples
         loss = R.backward(scene["means"], scene["quats"], scene["scales"], scene["opacities"], scene["sh"], viewmats, Ks, gt_image, randns,
                           v_samples=self.v_samples, zero_grads=False, raw=scene.get("raw"), w_rgb=self.rgb_w, w_depth=self.depth_w,
-                          w_dssim=self.dssim_w, w_normal=self.normal_w, w_isotropic=self.iso_w)
+                          w_dssim=self.dssim_w, w_normal=self.normal_w, w_isotropic=self.iso_w, bck_color=self.bck_color, bg=self.bg,
+                          mask=self.mask)
         return loss, self.sdf_loss
 
 
@@ -669,9 +717,11 @@ class GsSdfTrainer(GsSdfStep):
         down to the SH coefficients (the frozen structure's projection backward is skipped) and Adam over the SH groups. The structure's
         gradient segments are left for the caller to clear."""
         R, sc = self.R, self.scene
-        R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], viewmats, Ks, raw=sc["raw"])
+        R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], viewmats, Ks, raw=sc["raw"], bck_color=self.bck_color,
+                  bg=self.bg)
         loss = R.backward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], viewmats, Ks, gt_image, zero_grads=False,
-                          raw=sc["raw"], w_rgb=self.rgb_w, w_depth=0.0, w_dssim=self.dssim_w, projection_bwd=False)
+                          raw=sc["raw"], w_rgb=self.rgb_w, w_depth=0.0, w_dssim=self.dssim_w, projection_bwd=False, bck_color=self.bck_color,
+                          bg=self.bg, mask=self.mask)
         self.adam_sh()
         return loss
 

@@ -399,6 +399,48 @@ typedef struct gssdf_dssim_loss_args {
 size_t gssdf_dssim_workspace_bytes(int32_t C, int32_t image_width, int32_t image_height);
 int gssdf_dssim_loss(const gssdf_dssim_loss_args *a, gssdf_stream_t stream);
 
+/* f-15  Background and image mask of the photometric path (DESIGN 7o).
+ *     Background (NeuralGS::render, include/neural_gaussian/neural_gaussian.cpp:545-553): gssdf_render_post_fwd / _bwd with the
+ *     background composited into out_colors[..., 0:3] after the rasteriser, each step one fp32 rounding as ATen evaluates it:
+ *         bck_mode 0: c                      (black; the plain entry points)
+ *         bck_mode 1: c + (1 - alpha)        (white)
+ *         bck_mode 2: c + (1 - alpha) * bg   (bg [C,H,W,3], e.g. a fresh torch.rand per render)
+ *     Backward: the colour cotangent passes through; v_render_alphas additionally gets -(v_rgb . bg) (bg = 1 in mode 1). Expected
+ *     depth, alpha and the world normals are unchanged. GSSDF_EINVAL for bck_mode outside {0,1,2}, a NULL bg in mode 2, and every
+ *     check of the plain call. */
+typedef struct gssdf_render_post_bg_fwd_args {
+    gssdf_render_post_fwd_args post;
+    int32_t bck_mode;            /* 0 black, 1 white, 2 bg */
+    const float *bg;             /* [C,H,W,3] (mode 2) or NULL */
+} gssdf_render_post_bg_fwd_args;
+int gssdf_render_post_bg_fwd(const gssdf_render_post_bg_fwd_args *a, gssdf_stream_t stream);
+
+typedef struct gssdf_render_post_bg_bwd_args {
+    gssdf_render_post_bwd_args post;
+    int32_t bck_mode;
+    const float *bg;             /* [C,H,W,3] (mode 2) or NULL */
+} gssdf_render_post_bg_bwd_args;
+int gssdf_render_post_bg_bwd(const gssdf_render_post_bg_bwd_args *a, gssdf_stream_t stream);
+
+/* Image mask (loss::rgb_loss / loss::dssim_loss with a mask, include/optimizer/loss.cpp:22-47). mask [H,W,3] uint8, nonzero = 1, one
+ * mask for all C cameras (the reference holds one per dataset):
+ *     L1:    loss_out += w_rgb * sum |(rgb - gt) * m| / (3 C H W) + the unmasked depth term;  v_rgb = w_rgb / (3 C H W) * sgn(rgb - gt) * m
+ *            (the mean still runs over every element, as the reference's .mean())
+ *     DSSIM: loss_out += w_dssim * (1 - mean SSIM(rgb * m, gt * m));  v_rgb += m * d/d(rgb * m)
+ * With an all-ones mask both are bit-identical to the unmasked calls. GSSDF_EINVAL for a NULL mask and every check of the plain call;
+ * the DSSIM workspace is gssdf_dssim_workspace_bytes. */
+typedef struct gssdf_l1_loss_masked_args {
+    gssdf_l1_loss_args loss;
+    const uint8_t *mask;         /* [H,W,3] */
+} gssdf_l1_loss_masked_args;
+int gssdf_l1_loss_masked(const gssdf_l1_loss_masked_args *a, gssdf_stream_t stream);
+
+typedef struct gssdf_dssim_loss_masked_args {
+    gssdf_dssim_loss_args loss;
+    const uint8_t *mask;         /* [H,W,3] */
+} gssdf_dssim_loss_masked_args;
+int gssdf_dssim_loss_masked(const gssdf_dssim_loss_masked_args *a, gssdf_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * a9-a12  SDF branch: multiresolution hash-grid encoding + decoder MLP, first order.
  *     Replaces LocalMap::get_sdf (include/neural_net/local_map.cpp:87-103) = EncodingMap::encoding

@@ -14,7 +14,12 @@
 Frames live in pinned host memory (one asynchronous copy per iteration). Prints one JSON line per SH degree with the GPU's name and power
 limit read in the same run.
 
-  python tools/gs_train_bench.py [--sh 0,3] [--iters 4000] [--frames 60] [--window 50] [--rounds 4]
+--options instead times what the render background and the image mask cost: two trainers from the same SDF stage and splats, one with
+the defaults and one with bck_color=1 and a mask (a quarter of the frame masked out), run second-half joint iterations (no densification,
+so the splat count stays put) in alternating windows of --window iterations; prints the median and the spread (min, max) of the ms per
+iteration of each.
+
+  python tools/gs_train_bench.py [--sh 0,3] [--iters 4000] [--frames 60] [--window 50] [--rounds 4] [--options]
 """
 import argparse
 import json
@@ -80,6 +85,7 @@ def main():
     ap.add_argument("--sdf-iters", type=int, default=200)
     ap.add_argument("--window", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=4)
+    ap.add_argument("--options", action="store_true", help="time bck_color=1 + a mask against the defaults")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     pack = S.box_room_pack(dev, 120, ds_pt_num=2000, seed=0)  # the depth pack of the GPU tests (its resolution does not enter the render)
@@ -97,7 +103,7 @@ def main():
     del imgs_dev
     K = torch.tensor([[fx, 0, (W - 1) / 2.0], [0, fx, (H - 1) / 2.0], [0, 0, 1.0]])
     info = gpu_info()
-    def trainer(sh):
+    def trainer(sh, **kw):
         net = SD.SdfNet(dev, origin=frame["origin"], map_size=frame["map_size"], bce_isigma=1.0 / BCE_SIGMA, seed=1342)
         sdf = NS.SdfTrainer(net, tree, pack, args.sdf_iters, leaf_size=LEAF, bce_sigma=BCE_SIGMA, xyz_min=lo, xyz_max=hi, seed=5,
                             outlier_remove=True)
@@ -107,9 +113,30 @@ def main():
                                   map_origin=frame["origin"], sky=True, generator=torch.Generator(dev).manual_seed(0))
         n0 = int(sp["anchors"].shape[0])
         return GT.GsTrainer(sdf, sp, c2w, K, imgs, capacity=16 * n0, spatial_scale=0.5 * frame["inner_map_size"], gs_iter_step=args.iters,
-                            sh_degree=sh, outlier_remove=True), n0
+                            sh_degree=sh, outlier_remove=True, **kw), n0
 
     w, half = args.window, args.iters // 2
+    if args.options:
+        mask = torch.ones(H, W, dtype=torch.bool, device=dev)
+        mask[H // 4:3 * H // 4, W // 4:3 * W // 4] = False
+        for sh in [int(s) for s in args.sh.split(",")]:
+            runs = dict(defaults=trainer(sh)[0], bck_color_1_mask=trainer(sh, bck_color=1, mask=mask)[0])
+            for G in runs.values():
+                G.run_color_init()
+                G.start_rates()
+            ms = {k: [] for k in runs}
+            for r in range(2 * args.rounds + 1):
+                for k, G in runs.items():
+                    i0 = half + r * w
+                    t = ev_ms(lambda G=G, i0=i0: [G.step(j) for j in range(i0, min(i0 + w, args.iters))]) / w
+                    if r > 0:  # the first window of each is the warm-up
+                        ms[k].append(t)
+            stat = lambda v: dict(median=round(float(np.median(v)), 3), min=round(min(v), 3), max=round(max(v), 3))
+            print(json.dumps({"sh_degree": sh, "W": W, "H": H, "frames": args.frames, "splats": {k: G.T.N_live for k, G in runs.items()},
+                              "window": w, "windows": 2 * args.rounds, **{k + "_ms": stat(v) for k, v in ms.items()}, "gpu": info}), flush=True)
+            del runs
+            torch.cuda.empty_cache()
+        return
     for sh in [int(s) for s in args.sh.split(",")]:
         G, n0 = trainer(sh)
         torch.cuda.synchronize()
