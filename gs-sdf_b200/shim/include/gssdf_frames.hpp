@@ -1,0 +1,14 @@
+// libtorch entry point of the render path's 8-bit frames (gssdf_render_frames_u8, include/gssdf_b200.h; DESIGN 7p) for the reference's
+// NeuralSLAM::render_path (include/neural_mapping/neural_mapping.cpp:932-1200), in place of its per-view utils::tensor_to_cv_mat and
+// utils::apply_colormap_to_depth (INTEGRATION 3p). Implemented in shim/gssdf_frames.cpp; the same bytes as gssdf_b200.views.render_frames.
+#pragma once
+#include <torch/torch.h>
+
+#include <vector>
+
+namespace gssdf {
+// {color, depth, normal}: uint8 [C,H,W,3] CUDA tensors (RGB) of C rendered views, from out_colors [C,H,W,4] (RGB after the background
+// composite, expected depth in channel 3) and out_normals [C,H,W,3] (the world-frame rendered normal), float32 CUDA tensors; [H,W,4] and
+// [H,W,3] are read as one view. No host sync; the caller's cv::imwrite takes each view after a .cpu() and cv::cvtColor(RGB2BGR).
+std::vector<torch::Tensor> render_frames(const torch::Tensor &out_colors, const torch::Tensor &out_normals);
+}  // namespace gssdf

@@ -1431,6 +1431,41 @@ typedef struct gssdf_sdf_adapt_args {
 } gssdf_sdf_adapt_args;
 int gssdf_sdf_adapt(const gssdf_sdf_adapt_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-16  8-bit frames of rendered views.  Replaces the host composition of NeuralSLAM::render_path
+ *     (include/neural_mapping/neural_mapping.cpp:932-1200): utils::tensor_to_cv_mat of the colour, the depth and the normal * 0.5 + 0.5,
+ *     and utils::apply_colormap_to_depth with its defaults (include/utils/utils.cpp:250-283, utils.h:61-65) (DESIGN 7p). One call writes
+ *     the three frames of C views; no allocation, no host sync; every argument is checked before the first launch.
+ * ------------------------------------------------------------------------------------------ */
+/* Inputs (gssdf_render_post_fwd's / _bg_fwd's outputs): out_colors [C,H,W,4] (RGB after the background composite, expected depth in
+   channel 3), out_normals [C,H,W,3] (the world-frame rendered normal, render_results["render_normal"][0]). Outputs: three uint8
+   [C,H,W,3] images in RGB order (the file writer's cvtColor to BGR is left to it). Every `_rn` is one IEEE rounding.
+     trunc8(x)  = (uint8)(int64) fl_rn(clamp(x, 0, 1) * 255)   (ATen's clamp / mul / .to(kUInt8) on the device; a NaN gives 0)
+     color      = trunc8(rgb)
+     normal     = trunc8(fl_rn(fl_rn(n * 0.5) + 0.5))
+     depth, per view:
+       mm       = saturate_u16(round(fl_rn(d * 1000)))          (convertTo(CV_16UC1, 1000))
+       near/far = min / max of mm over the pixels with mm > 0    (cv::minMaxLoc with the mask; (0, 0) when there are none)
+       alpha    = 1 / (far - near + 1e-10),  beta = -near * alpha            (fp64: the MatExpr (m - near) / (...) is one convertTo)
+       t        = fma_rn((float)mm, (float)alpha, (float)beta), or 1 where mm == 0
+       q        = saturate_u8(round(fl_rn(t * 255)))             (convertTo(CV_8UC1, 255))
+       depth    = TURBO[q]                                      (cv::applyColorMap, COLORMAP_TURBO, as RGB)
+   round() is OpenCV's cvRound (to nearest, ties to even); a value outside int32 or a NaN converts to INT_MIN and saturates to 0.
+   Bit-identical from run to run and between one call of C views and C calls of one view.
+   GSSDF_EINVAL before any launch for C outside [0, 65535], W or H < 1, W H > 2^29, a NULL pointer, out_colors not 16-byte or
+   out_normals not 4-byte aligned, or a workspace that is too small. C == 0 is a no-op. */
+typedef struct gssdf_render_frames_args {
+    int32_t C, W, H;
+    const float *out_colors;      /* [C,H,W,4] */
+    const float *out_normals;     /* [C,H,W,3] */
+    uint8_t *color, *depth, *normal;  /* [C,H,W,3] each, overwritten */
+    void *workspace;              /* >= gssdf_render_frames_workspace_bytes(C, W, H) */
+    size_t workspace_bytes;
+} gssdf_render_frames_args;
+/* 0 for C outside [0, 65535], W or H < 1 or W H > 2^29 */
+size_t gssdf_render_frames_workspace_bytes(int32_t C, int32_t W, int32_t H);
+int gssdf_render_frames_u8(const gssdf_render_frames_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
