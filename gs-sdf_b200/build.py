@@ -13,7 +13,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 
 def build(verbose=False, force=False):
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "adam.cuh"), os.path.join(CSRC, "sdf_grid.cuh"), os.path.join(CSRC, "conic.cuh"), os.path.join(CSRC, "sdf_loss.cuh"), os.path.join(CSRC, "mc_table.h"), os.path.join(CSRC, "octree_query.cuh"), os.path.join(CSRC, "morton.cuh"), os.path.join(HERE, "..", "include", "gssdf_b200.h")]
+    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "adam.cuh"), os.path.join(CSRC, "sdf_grid.cuh"), os.path.join(CSRC, "conic.cuh"), os.path.join(CSRC, "sdf_loss.cuh"), os.path.join(CSRC, "mc_table.h"), os.path.join(CSRC, "octree_query.cuh"), os.path.join(CSRC, "morton.cuh"), os.path.join(CSRC, "depth_normal.cuh"), os.path.join(HERE, "..", "include", "gssdf_b200.h")]
     if not force and os.path.exists(OUT) and all(os.path.getmtime(d) <= os.path.getmtime(OUT) for d in deps):
         return OUT
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

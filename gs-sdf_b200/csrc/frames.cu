@@ -7,9 +7,13 @@
 // min / max: the result does not depend on the order). Pass 2 maps every pixel through the view's (near, far) and the TURBO table.
 // Each thread owns 4 consecutive pixels; when a view's pixel count is a multiple of 4 and the buffers are aligned, those are 12 output
 // bytes = three 32-bit stores per image, and the inputs are float4 loads.
+//
+// The depth-to-normal frame of export_test_image (include/neural_mapping/neural_mapping.cpp:1288-1310) is one more launch of its own
+// (gssdf_render_depth_normal_u8): it reads a 3x3 neighbourhood of the depth, so it tiles the image as the normal-consistency loss does.
 #include <cmath>
 
 #include "common.cuh"
+#include "depth_normal.cuh"
 
 namespace gssdf {
 namespace {
@@ -207,6 +211,29 @@ frames_pass2_kernel(int64_t HW, const uint16_t *__restrict__ mm, const uint32_t 
     }
 }
 
+// The depth-to-normal frame: one 32x8 pixel tile per CTA stages its halo-1 world points (depth_normal.cuh, the normal-consistency loss's
+// staging and stencil), then each thread writes trunc8(fl(fl(n * alpha) * 0.5) + 0.5) of its pixel, n = 0 on the border rows / columns.
+constexpr int kDnX = 32, kDnY = 8;
+
+__global__ void __launch_bounds__(kDnX * kDnY) depth_normal_kernel(const gssdf_render_depth_normal_args a) {
+    __shared__ float sP[kDnY + 2][kDnX + 2][3];
+    const int W = a.W, H = a.H, cam = blockIdx.z;
+    const int bx = blockIdx.x * kDnX, by = blockIdx.y * kDnY;
+    const DnCamera cm = dn_camera(a.viewmats, a.Ks, cam);
+    const int64_t img = (int64_t)cam * H * W;
+    dn_stage<kDnY + 2, kDnX + 2>(sP, cm, a.depth, a.depth_stride, img, W, H, bx - 1, by - 1, threadIdx.y * kDnX + threadIdx.x, kDnX * kDnY);
+    __syncthreads();
+    const int gx = bx + threadIdx.x, gy = by + threadIdx.y;
+    if (gx >= W || gy >= H) return;
+    float n[3] = {0.f, 0.f, 0.f};
+    if (gx >= 1 && gx <= W - 2 && gy >= 1 && gy <= H - 2) dn_normal<kDnX + 2>(sP, threadIdx.y + 1, threadIdx.x + 1, n);
+    const int64_t pix = img + (int64_t)gy * W + gx;
+    const float alpha = __ldg(a.render_alphas + pix);
+    // depth2normal * alpha, * 0.5f, + 0.5f: three ATen ops, three roundings
+    put3(a.normal + pix * 3, to_u8_trunc(__fadd_rn(__fmul_rn(__fmul_rn(n[0], alpha), 0.5f), 0.5f)),
+         to_u8_trunc(__fadd_rn(__fmul_rn(__fmul_rn(n[1], alpha), 0.5f), 0.5f)), to_u8_trunc(__fadd_rn(__fmul_rn(__fmul_rn(n[2], alpha), 0.5f), 0.5f)));
+}
+
 bool size_ok(int32_t C, int32_t W, int32_t H) {
     return C >= 0 && C <= kMaxViews && W >= 1 && H >= 1 && (int64_t)W * H <= ((int64_t)1 << 31) / kPix;
 }
@@ -245,5 +272,20 @@ extern "C" int gssdf_render_frames_u8(const gssdf_render_frames_args *a, gssdf_s
     if (vec) frames_pass2_kernel<true><<<grid, kThreads, 0, st>>>(HW, w.mm, w.vmin, w.vmax, a->depth);
     else frames_pass2_kernel<false><<<grid, kThreads, 0, st>>>(HW, w.mm, w.vmin, w.vmax, a->depth);
     GSSDF_LAUNCH_OK("frames_pass2_kernel");
+    return GSSDF_OK;
+}
+
+extern "C" int gssdf_render_depth_normal_u8(const gssdf_render_depth_normal_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "render_depth_normal: null args");
+    GSSDF_REQUIRE(size_ok(a->C, a->W, a->H) && a->H <= kMaxViews * kDnY, GSSDF_EINVAL, "render_depth_normal: bad batch %d x %d x %d", a->C,
+                  a->W, a->H);
+    if (a->C == 0) return GSSDF_OK;
+    GSSDF_REQUIRE(a->viewmats && a->Ks && a->depth && a->render_alphas && a->normal, GSSDF_EINVAL, "render_depth_normal: null pointer");
+    GSSDF_REQUIRE(a->depth_stride >= 1, GSSDF_EINVAL, "render_depth_normal: depth_stride %d < 1", a->depth_stride);
+    GSSDF_REQUIRE(aligned(a->viewmats, 4) && aligned(a->Ks, 4) && aligned(a->depth, 4) && aligned(a->render_alphas, 4), GSSDF_EINVAL,
+                  "render_depth_normal: float inputs must be 4-byte aligned");
+    const dim3 grid(cdiv(a->W, kDnX), cdiv(a->H, kDnY), a->C), block(kDnX, kDnY);
+    depth_normal_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(*a);
+    GSSDF_LAUNCH_OK("depth_normal_kernel");
     return GSSDF_OK;
 }

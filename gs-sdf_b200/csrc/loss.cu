@@ -17,6 +17,7 @@
 // through shared memory: ~180 shared-memory wavefronts per channel-pixel incl. 2-way bank conflicts and seven barriers per tile,
 // 0.17 ms per direction at 1080p; this one needs 29.)
 #include "common.cuh"
+#include "depth_normal.cuh"
 
 namespace gssdf {
 
@@ -327,7 +328,8 @@ extern "C" int gssdf_dssim_loss_masked(const gssdf_dssim_loss_masked_args *a, gs
 // of the rendered depth map (sensor::depth_to_normal, include/utils/sensor_utils/cameras.hpp:176-226), loss + both cotangents in one
 // tile kernel. A 32x8 pixel tile stages the world points P = dir_w * depth of its halo-2 neighbourhood in shared memory, evaluates the
 // stencil normal and dL/d(cross product) on the halo-1 ring, then every pixel GATHERS its depth gradient from its four neighbours'
-// stencils (deterministic; the autograd graph of the reference scatters through index/cat/cross/normalize backward kernels).
+// stencils (deterministic; the autograd graph of the reference scatters through index/cat/cross/normalize backward kernels). The
+// staging and the stencil normal are depth_normal.cuh's, which the depth-to-normal frame (frames.cu) shares.
 // ---------------------------------------------------------------------------------------------------------------------------------
 namespace gssdf {
 
@@ -340,25 +342,9 @@ __global__ void __launch_bounds__(kNcX * kNcY) normal_consistency_kernel(const g
     const int W = a.image_width, H = a.image_height, cam = blockIdx.z;
     const int tid = threadIdx.y * kNcX + threadIdx.x;
     const int bx = blockIdx.x * kNcX, by = blockIdx.y * kNcY;
-    const float *V = a.viewmats + 16 * cam, *K = a.Ks + 9 * cam;
-    const float ifx = 1.f / K[0], ify = 1.f / K[4], cx = K[2], cy = K[5];
+    const DnCamera cm = dn_camera(a.viewmats, a.Ks, cam);
     const int64_t img = (int64_t)cam * H * W;
-    auto dir_w = [&](int gx, int gy, float d[3]) {  // rot * zdir with rot = R^T of the world->camera view matrix
-        const float zx = ((float)gx + 0.5f - cx) * ifx, zy = ((float)gy + 0.5f - cy) * ify;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) d[k] = V[0 * 4 + k] * zx + V[1 * 4 + k] * zy + V[2 * 4 + k];
-    };
-    for (int e = tid; e < (kNcY + 4) * (kNcX + 4); e += kNcX * kNcY) {
-        const int r = e / (kNcX + 4), c = e % (kNcX + 4), gx = bx + c - 2, gy = by + r - 2;
-        float p[3] = {0.f, 0.f, 0.f};
-        if (gx >= 0 && gx < W && gy >= 0 && gy < H) {
-            float d[3];
-            dir_w(gx, gy, d);
-            const float z = __ldg(a.depth + (img + (int64_t)gy * W + gx) * a.depth_stride);
-            p[0] = d[0] * z; p[1] = d[1] * z; p[2] = d[2] * z;  // (+ pos: cancels in the differences)
-        }
-        sP[r][c][0] = p[0]; sP[r][c][1] = p[1]; sP[r][c][2] = p[2];
-    }
+    dn_stage<kNcY + 4, kNcX + 4>(sP, cm, a.depth, a.depth_stride, img, W, H, bx - 2, by - 2, tid, kNcX * kNcY);
     __syncthreads();
     float part = 0.f;
     for (int e = tid; e < (kNcY + 2) * (kNcX + 2); e += kNcX * kNcY) {
@@ -371,14 +357,8 @@ __global__ void __launch_bounds__(kNcX * kNcY) normal_consistency_kernel(const g
             float grn[3] = {0.f, 0.f, 0.f};
             float dot = 0.f;
             if (gx >= 1 && gx <= W - 2 && gy >= 1 && gy <= H - 2) {  // interior: depth_point_to_normal fills [1:-1, 1:-1]
-                const int pr = r + 1, pc = c + 1;
-                float va[3], vb[3];
-#pragma unroll
-                for (int k = 0; k < 3; ++k) { va[k] = sP[pr + 1][pc][k] - sP[pr - 1][pc][k]; vb[k] = sP[pr][pc + 1][k] - sP[pr][pc - 1][k]; }
-                const float cr[3] = {va[1] * vb[2] - va[2] * vb[1], va[2] * vb[0] - va[0] * vb[2], va[0] * vb[1] - va[1] * vb[0]};
-                const float nrm = sqrtf(cr[0] * cr[0] + cr[1] * cr[1] + cr[2] * cr[2]);
-                const float den = fmaxf(nrm, 1e-12f);  // F::normalize eps
-                const float n[3] = {cr[0] / den, cr[1] / den, cr[2] / den};
+                float n[3];
+                const float nrm = dn_normal<kNcX + 4>(sP, r + 1, c + 1, n);
                 const float rn[3] = {__ldg(a.out_normals + 3 * pix), __ldg(a.out_normals + 3 * pix + 1), __ldg(a.out_normals + 3 * pix + 2)};
                 dot = alpha * (n[0] * rn[0] + n[1] * rn[1] + n[2] * rn[2]);
                 if (isfinite(dot)) {  // nan_to_num: value 0 and zero gradient where the product is not finite
@@ -428,7 +408,7 @@ __global__ void __launch_bounds__(kNcX * kNcY) normal_consistency_kernel(const g
         add(pr, pc - 1, false, 1.f);
         add(pr, pc + 1, false, -1.f);
         float d[3];
-        dir_w(gx, gy, d);
+        dn_dir_w(cm, gx, gy, d);
         const float gz = gP[0] * d[0] + gP[1] * d[1] + gP[2] * d[2];
         a.v_depth[(img + (int64_t)gy * W + gx) * a.v_depth_stride] += gz;
     }

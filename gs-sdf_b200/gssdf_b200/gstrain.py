@@ -81,18 +81,22 @@ class GsTrainer:
         0 black, 1 white (FAST-LIVO2, Oxford Spires, HKU), 2 a uniform random image drawn before every render from a device generator of
         its own (`bg_gen`, seeded from `seed`; the splat samples' draws stay those of modes 0 and 1).
     mask: the dataset's image mask, bool or uint8 [H,W], [H,W,1] or [H,W,3] on the device (nonzero = keep), applied to every frame's L1
-        and DSSIM terms as loss::rgb_loss / dssim_loss do."""
+        and DSSIM terms as loss::rgb_loss / dssim_loss do.
+    depth_type: the config's `depth_type` (k_depth_type), the depth the normal-consistency term differentiates from iteration
+        refine_gs_struct_start_iter on: 0 the expected depth, any other int the rasteriser's median depth (bounded scenes; the COLMAP
+        configurations set 1 or 3)."""
 
     def __init__(self, sdf, splats, poses, K, images, *, capacity, spatial_scale, gs_iter_step=30000, color_init=True,
                  detach_sdf_grad=False, refine_gs_struct_start_iter=3000, rgb_weight=0.8, dssim_weight=0.2, render_normal_weight=0.01,
                  isotropic_weight=0.05, gs_sdf_weight=1e-3, visible_thr=0.1, outlier_remove=False, outlier_dist=0.05,
                  outlier_removal_interval=2000, sh_degree=3, sh_degree_interval=1000, densify=None, isect_cap=None, seed=0, bck_color=0,
-                 mask=None):
+                 mask=None, depth_type=0):
         dev = sdf.dev
         if not (gs_iter_step >= 1 and outlier_removal_interval >= 1 and sh_degree_interval >= 1):
             raise ValueError("GsTrainer: gs_iter_step, outlier_removal_interval and sh_degree_interval must be >= 1")
         hw = tuple(images.shape[1:3]) if isinstance(images, torch.Tensor) and images.dim() == 4 else (None, None)
         RD.check_photometric("GsTrainer", bck_color, mask, hw[0], hw[1], dev)
+        RD.check_depth_type("GsTrainer", depth_type)
         for k in ("xyz", "origin", "direction", "depth"):
             if not sdf.pack[k].is_cuda:
                 raise ValueError(f"GsTrainer: the SdfTrainer's pack[{k!r}] must be on the device")
@@ -111,6 +115,7 @@ class GsTrainer:
         self.sdf, self.dev, self.iters, self.train_num = sdf, dev, int(gs_iter_step), n_frames
         self.color_init, self.detach = bool(color_init), bool(detach_sdf_grad)
         self.refine_struct_start, self.normal_w = int(refine_gs_struct_start_iter), float(render_normal_weight)
+        self.depth_type = depth_type
         self.outlier_remove, self.outlier_dist, self.outlier_interval = bool(outlier_remove), float(outlier_dist), int(outlier_removal_interval)
         self.spatial_scale = float(spatial_scale)
         self.viewmats = torch.linalg.inv(poses.to(torch.float64)).to(torch.float32).to(dev).contiguous()
@@ -123,7 +128,8 @@ class GsTrainer:
                                      sh_degree=sh_degree, bce_sigma=sdf.bce_sigma, eikonal_weight=sdf.eik_w, gs_sdf_weight=gs_sdf_weight,
                                      visible_thr=visible_thr, mlp_mode=1, eikonal_mode=1, align_weight=sdf.align_w, rgb_weight=rgb_weight,
                                      dssim_weight=dssim_weight, depth_weight=0.0, normal_weight=0.0, isotropic_weight=isotropic_weight,
-                                     spatial_scale=self.spatial_scale, n_live=n0, delta_dev=sdf.std_dev, bck_color=bck_color, mask=mask)
+                                     spatial_scale=self.spatial_scale, n_live=n0, delta_dev=sdf.std_dev, bck_color=bck_color, mask=mask,
+                                     depth_type=depth_type)
         T.origin, T.inv_size, T.bce_isigma = net.origin, net.inv_size, sdf.bce_isigma
         T.set_octree(sdf.rs.tree)
         n_sdf = sdf.n_table + sdf.n_mlp

@@ -32,6 +32,15 @@ def check_photometric(who, bck_color, mask, H, W, device):
         raise ValueError(f"{who}: mask must be on {dev}, got {mask.device}")
 
 
+def check_depth_type(who, depth_type):
+    """k_depth_type, the depth the normal-consistency term and the depth-to-normal frame differentiate (neural_mapping.cpp:248-252,
+    config/base.yaml:43): 0 the expected depth, any other int the rasteriser's median depth (bounded scenes; the COLMAP configurations'
+    `depth_type`). Returns True for the median."""
+    if isinstance(depth_type, bool) or not isinstance(depth_type, int):
+        raise ValueError(f"{who}: depth_type must be an int (0: expected depth, otherwise the median depth), got {depth_type!r}")
+    return depth_type != 0
+
+
 def expand_mask(mask, H, W):
     """A checked mask as the masked loss kernels read it: uint8 [H,W,3], nonzero -> 1 (the reference's bool mask)."""
     return None if mask is None else mask.reshape(H, W, -1).ne(0).to(torch.uint8).expand(H, W, 3).contiguous()
@@ -132,11 +141,13 @@ class SplatRenderer:
     # -- loss + backward -----------------------------------------------------------------------
     def backward(self, means, quats, scales, opacities, sh, viewmats, Ks, gt, randns=None, w_rgb=1.0, w_depth=0.1, v_samples=None,
                  zero_grads=True, raw=None, w_dssim=0.0, w_normal=0.0, w_isotropic=0.0, before_projection_bwd=None, projection_bwd=True,
-                 bck_color=0, bg=None, mask=None):
+                 bck_color=0, bg=None, mask=None, median_depth=False):
         """With raw parameters the flat gradient holds dL/d(offsets|quats|log-scales|logits|features_dc|features_rest); the SH segment
         keeps its [N,K,3] size, laid out as dc [N,1,3] followed by rest [N,K-1,3]. projection_bwd=False stops after the SH backward (the
         structure is frozen: only the colour gradient is wanted). bck_color / bg: those of the forward; mask: uint8 [H,W,3]
-        (expand_mask) multiplying both images in the L1 and DSSIM terms (loss::rgb_loss / dssim_loss with a mask)."""
+        (expand_mask) multiplying both images in the L1 and DSSIM terms (loss::rgb_loss / dssim_loss with a mask). median_depth: the
+        normal term differentiates render_median instead of the expected depth (check_depth_type); its depth cotangent then enters the
+        rasteriser backward as v_render_median."""
         C, W, H, cap = self.C, self.W, self.H, self.cap
         off, rest = (raw["offsets"], raw["sh_rest"]) if raw else (None, None)
         N, K = self.N, self.K
@@ -154,8 +165,14 @@ class SplatRenderer:
                 cabi.dssim_loss(C, W, H, self.out_colors, gt, w_dssim, self.loss, self.v_out_colors, self.loss_ws)
             else:
                 cabi.dssim_loss_masked(C, W, H, self.out_colors, gt, w_dssim, self.loss, self.v_out_colors, self.loss_ws, mask)
-        if w_normal > 0:  # normal consistency between the rendered normals and the normals of the expected-depth map
-                          # (neural_mapping.cpp:243-266): adds to the ED cotangent (channel 3) and overwrites the normal cotangent
+        if w_normal > 0 and median_depth:  # the same term on the median depth (k_depth_type != 0): the kernel adds to v_render_median,
+                                           # which is zero outside this branch
+            self.v_r["median"].zero_()
+            cabi.normal_consistency_loss(C, W, H, viewmats, Ks, self.r["render_median"], 1, self.r["render_alphas"], self.out_normals,
+                                         w_normal, self.loss, v_depth=self.v_r["median"], v_depth_stride=1, v_out_normals=self.v_out_normals)
+            self._v_normals_dirty = self._v_median_dirty = True
+        elif w_normal > 0:  # normal consistency between the rendered normals and the normals of the expected-depth map
+                            # (neural_mapping.cpp:243-266): adds to the ED cotangent (channel 3) and overwrites the normal cotangent
             cabi.normal_consistency_loss(C, W, H, viewmats, Ks, self.out_colors.data_ptr() + 12, 4, self.r["render_alphas"], self.out_normals,
                                          w_normal, self.loss, v_depth=self.v_out_colors.data_ptr() + 12, v_depth_stride=4,
                                          v_out_normals=self.v_out_normals)
@@ -163,6 +180,9 @@ class SplatRenderer:
         elif getattr(self, "_v_normals_dirty", False):
             self.v_out_normals.zero_()
             self._v_normals_dirty = False
+        if not (w_normal > 0 and median_depth) and getattr(self, "_v_median_dirty", False):
+            self.v_r["median"].zero_()
+            self._v_median_dirty = False
         if w_isotropic > 0:  # isotropic regulariser on the visible splats' (x, y) scales (neural_mapping.cpp:268-276)
             cabi.isotropic_loss(self.N, cap, self.counts, self.p["gaussian_ids"], scales, raw is not None, w_isotropic, self.loss,
                                 self.v_scales)
@@ -229,13 +249,15 @@ class GsSdfStep:
     def __init__(self, N, K, W, H, device, isect_cap, sdf_net_cfg, n_ray_samples=32768, sh_degree=3, origin=(0.0, 0.0, 0.0),
                  map_size=14.0, bce_sigma=0.1, delta=None, eikonal_weight=0.1, gs_sdf_weight=1e-3, visible_thr=0.1, mlp_mode=None,
                  eikonal_mode=None, align_weight=0.1, rgb_weight=0.8, dssim_weight=0.2, depth_weight=0.1, normal_weight=0.0,
-                 isotropic_weight=0.0, delta_dev=None, bck_color=0, mask=None):
+                 isotropic_weight=0.0, delta_dev=None, bck_color=0, mask=None, depth_type=0):
         """delta_dev: float32 CUDA tensor [1] read by every SDF call of [A] and [C] in place of the host scalar `delta` (the sample std the
         SDF stage adapts on the device, nsdf.SdfTrainer.std_dev); the ray-site forward then also evaluates the base variant into ray_y1.
         bck_color (k_bck_color: 0 black, 1 white, 2 random) and mask (bool / uint8 [H,W], [H,W,1] or [H,W,3] on the device, one for every
         frame): the render's background and the photometric loss's image mask (DESIGN 7o), in the joint step and in color_step. With
-        bck_color 2 the render composites self.bg [1,H,W,3], which the caller fills before every render (gstrain.GsTrainer draws it)."""
+        bck_color 2 the render composites self.bg [1,H,W,3], which the caller fills before every render (gstrain.GsTrainer draws it).
+        depth_type (k_depth_type): the depth of the normal-consistency term, 0 the expected depth, any other int the median depth."""
         check_photometric("GsSdfStep", bck_color, mask, H, W, device)
+        self.median_depth = check_depth_type("GsSdfStep", depth_type)
         self.R = SplatRenderer(N, K, 1, W, H, device, isect_cap, sh_degree=sh_degree)
         self.bck_color, self.mask = int(bck_color), expand_mask(mask, H, W)
         self.bg = torch.zeros(1, H, W, 3, dtype=torch.float32, device=device) if self.bck_color == 2 else None
@@ -446,7 +468,7 @@ class GsSdfStep:
             loss = R.backward(scene["means"], scene["quats"], scene["scales"], scene["opacities"], scene["sh"], viewmats, Ks, gt_image, randns,
                               v_samples=self.v_samples, zero_grads=False, raw=scene.get("raw"), w_rgb=self.rgb_w, w_depth=self.depth_w,
                               w_dssim=self.dssim_w, w_normal=self.normal_w, w_isotropic=self.iso_w, before_projection_bwd=wait_c,
-                              bck_color=self.bck_color, bg=self.bg, mask=self.mask)
+                              bck_color=self.bck_color, bg=self.bg, mask=self.mask, median_depth=self.median_depth)
             return loss, self.sdf_loss
         cabi.sdf_gate_count(cap, self.n_gate, visibilities=R.r["visibilities"], visible_thr=self.vis_thr, valid_mask=self.valid_mask,
                             n_live=n_live)
@@ -484,7 +506,7 @@ class GsSdfStep:
         loss = R.backward(scene["means"], scene["quats"], scene["scales"], scene["opacities"], scene["sh"], viewmats, Ks, gt_image, randns,
                           v_samples=self.v_samples, zero_grads=False, raw=scene.get("raw"), w_rgb=self.rgb_w, w_depth=self.depth_w,
                           w_dssim=self.dssim_w, w_normal=self.normal_w, w_isotropic=self.iso_w, bck_color=self.bck_color, bg=self.bg,
-                          mask=self.mask)
+                          mask=self.mask, median_depth=self.median_depth)
         return loss, self.sdf_loss
 
 

@@ -2,7 +2,8 @@
 
 `render_views` renders batches of consecutive frames of one resolution through `render.SplatRenderer` (one renderer per resolution,
 per-view intrinsics) and turns each batch's float outputs into the colour, depth-colourmap and normal images on the device
-(gssdf_render_frames_u8), so only 9 bytes a pixel come back to the host. `render_path` writes them in the reference's layout.
+(gssdf_render_frames_u8), so only 9 bytes a pixel come back to the host; on request it adds export_test_image's depth-to-normal frame
+(gssdf_render_depth_normal_u8). `render_path` writes them in the reference's layout.
 `load_camera_spec` reads the render camera spec of the node's `render` mode (render_camera_spec_v1)."""
 import ctypes as C
 import os
@@ -13,7 +14,7 @@ import torch
 
 from . import cabi
 from ._lib import check, lib, make_args
-from .render import SplatRenderer, check_photometric
+from .render import SplatRenderer, check_depth_type, check_photometric
 
 # intersection capacity of a new renderer, per splat and view; a batch that needs more renders again at the counted size
 ISECT_PER_SPLAT = 16
@@ -104,6 +105,31 @@ def render_frames(out_colors, out_normals, ws=None, out=None):
     return tuple(out)
 
 
+def render_depth_normal(depth, render_alphas, viewmats, Ks, out=None):
+    """gssdf_render_depth_normal_u8: export_test_image's depth-to-normal frame, uint8 [C,H,W,3] (RGB) on the device, i.e.
+    tensor_to_cv_mat(depth_to_normal(depth) * alpha * 0.5 + 0.5) (include/gssdf_b200.h states the arithmetic). depth: SplatRenderer's
+    out_colors [C,H,W,4] (the expected depth in channel 3: depth_type 0) or its r["render_median"] [C,H,W,1] (any other depth_type);
+    render_alphas [C,H,W,1]; viewmats [C,4,4] world->camera and Ks [C,3,3]; float32 CUDA tensors. out: a preallocated frame to write."""
+    for t, name in ((depth, "depth"), (render_alphas, "render_alphas"), (viewmats, "viewmats"), (Ks, "Ks")):
+        cabi._req(t, torch.float32, name)
+    if depth.dim() != 4 or depth.shape[3] not in (1, 4):
+        raise ValueError(f"gssdf_b200: depth must be out_colors [C,H,W,4] or render_median [C,H,W,1], got {tuple(depth.shape)}")
+    Cn, H, W = (int(s_) for s_ in depth.shape[:3])
+    if (tuple(render_alphas.shape) != (Cn, H, W, 1) or tuple(viewmats.shape) != (Cn, 4, 4) or tuple(Ks.shape) != (Cn, 3, 3)):
+        raise ValueError(f"gssdf_b200: render_alphas must be [{Cn},{H},{W},1], viewmats [{Cn},4,4] and Ks [{Cn},3,3], got "
+                         f"{tuple(render_alphas.shape)}, {tuple(viewmats.shape)} and {tuple(Ks.shape)}")
+    if out is None:
+        out = torch.empty(Cn, H, W, 3, dtype=torch.uint8, device=depth.device)
+    cabi._req(out, torch.uint8, "frame")
+    if tuple(out.shape) != (Cn, H, W, 3):
+        raise ValueError(f"gssdf_b200: the frame buffer must be [{Cn},{H},{W},3], got {tuple(out.shape)}")
+    stride = int(depth.shape[3])
+    a = make_args("gssdf_render_depth_normal_args", C=Cn, W=W, H=H, viewmats=viewmats, Ks=Ks,
+                  depth=depth.data_ptr() + 4 * (stride - 1), depth_stride=stride, render_alphas=render_alphas, normal=out)
+    check(lib().gssdf_render_depth_normal_u8(C.byref(a), cabi._stream()))
+    return out
+
+
 # ---- rendering at any camera ---------------------------------------------------------------------------------------------------------
 def world_to_camera(pose_c2w):
     """NeuralGS::render's world->camera matrix (neural_gaussian.cpp:509-517): [R^T, -R^T t; 0 0 0 1] in fp32 from a camera->world
@@ -143,12 +169,15 @@ def _scene(splats, sh_degree, dev):
     return scene, N, K
 
 
-def render_views(splats, poses_c2w, cameras, *, sh_degree, bck_color=0, near=0.05, far=300.0, batch=8, generator=None):
+def render_views(splats, poses_c2w, cameras, *, sh_degree, bck_color=0, near=0.05, far=300.0, batch=8, generator=None, depth_normal=None):
     """Yields, in frame order, dict(color=, depth=, normal=) of uint8 [H,W,3] host tensors (RGB) per camera->world pose: the frames
     NeuralSLAM::render_path writes. splats: the raw NeuralGS parameters as GsTrainer.state()["splats"] or io.load_ply_to_gs give them,
     on the CUDA device to render on; poses_c2w [F,4,4] (or [F,3,4]); cameras: one (W, H, K [3,3]) for every frame or a list of F.
     Consecutive frames of one (W, H) render together, up to `batch` views per call; opacities through the sigmoid, SH up to sh_degree,
-    bck_color 0 black, 1 white, 2 a uniform random image per view drawn from `generator` (a CUDA generator, or torch's default)."""
+    bck_color 0 black, 1 white, 2 a uniform random image per view drawn from `generator` (a CUDA generator, or torch's default).
+    depth_normal: None for no depth-to-normal frame; else the training's depth_type (0: of the expected depth, any other int: of the
+    median depth), and each dict gains depth2normal=, export_test_image's mid/depth2normal_* frame (render_depth_normal)."""
+    median = None if depth_normal is None else check_depth_type("render_views", depth_normal)
     dev = splats["anchors"].device
     if dev.type != "cuda":
         raise ValueError("render_views: the splats must be on a CUDA device")
@@ -187,7 +216,9 @@ def render_views(splats, poses_c2w, cameras, *, sh_degree, bck_color=0, near=0.0
             R.forward(scene["means"], scene["quats"], scene["scales"], scene["opacities"], scene["sh"], vm, Ks, raw=scene["raw"],
                       bck_color=bck_color, bg=bg)
             frames = render_frames(R.out_colors, R.out_normals, ws)
-            host = [torch.empty(n, H, W, 3, dtype=torch.uint8, pin_memory=True) for _ in range(3)]
+            if median is not None:
+                frames += (render_depth_normal(R.r["render_median"] if median else R.out_colors, R.r["render_alphas"], vm, Ks),)
+            host = [torch.empty(n, H, W, 3, dtype=torch.uint8, pin_memory=True) for _ in frames]
             for h, d in zip(host, frames):
                 h.copy_(d[:n], non_blocking=True)
             cnt = R.read_counts()  # synchronises: the frames are on the host after this
@@ -200,7 +231,10 @@ def render_views(splats, poses_c2w, cameras, *, sh_degree, bck_color=0, near=0.0
                                    f"(at most {need})")
             R = renderers[(W, H)] = SplatRenderer(N, K, C_, W, H, dev, need, near=near, far=far, sh_degree=sh_degree)
         for v in range(n):
-            yield dict(color=host[0][v], depth=host[1][v], normal=host[2][v])
+            fr = dict(color=host[0][v], depth=host[1][v], normal=host[2][v])
+            if median is not None:
+                fr["depth2normal"] = host[3][v]
+            yield fr
 
 
 def render_path(splats, poses_c2w, cameras, out_dir, names=None, **kw):

@@ -1,4 +1,5 @@
-// gssdf::render_frames (shim/include/gssdf_frames.hpp) over the C ABI's gssdf_render_frames_u8, as gssdf_b200.views.render_frames does it.
+// gssdf::render_frames and gssdf::render_depth_normal_frames (shim/include/gssdf_frames.hpp) over the C ABI's gssdf_render_frames_u8 and
+// gssdf_render_depth_normal_u8, as gssdf_b200.views.render_frames and .render_depth_normal do it.
 #include "gssdf_frames.hpp"
 
 #include <ATen/cuda/CUDAContext.h>
@@ -42,5 +43,29 @@ std::vector<torch::Tensor> gssdf::render_frames(const torch::Tensor &out_colors,
     a.color = out[0].data_ptr<uint8_t>(), a.depth = out[1].data_ptr<uint8_t>(), a.normal = out[2].data_ptr<uint8_t>();
     a.workspace = ws.data_ptr(), a.workspace_bytes = (size_t)ws.numel();
     check(gssdf_render_frames_u8(&a, reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream())));
+    return out;
+}
+
+torch::Tensor gssdf::render_depth_normal_frames(const torch::Tensor &depth, const torch::Tensor &render_alphas, const torch::Tensor &viewmats,
+                                                const torch::Tensor &Ks) {
+    torch::NoGradGuard no_grad;
+    for (const torch::Tensor *t : {&depth, &render_alphas, &viewmats, &Ks}) {
+        TORCH_CHECK(t->is_cuda() && t->device() == depth.device(), "depth, render_alphas, viewmats and Ks must be CUDA tensors on one device");
+        TORCH_CHECK(t->scalar_type() == torch::kFloat, "depth, render_alphas, viewmats and Ks must be float32");
+    }
+    const torch::Tensor d = (depth.dim() == 3 ? depth.unsqueeze(0) : depth).contiguous();
+    TORCH_CHECK(d.dim() == 4 && (d.size(3) == 4 || d.size(3) == 1), "depth must be out_colors [C,H,W,4] or render_median [C,H,W,1]");
+    const int64_t C = d.size(0), H = d.size(1), W = d.size(2);
+    const torch::Tensor al = render_alphas.reshape({C, H, W, 1}).contiguous();
+    const torch::Tensor vm = viewmats.reshape({C, 4, 4}).contiguous(), K = Ks.reshape({C, 3, 3}).contiguous();
+    const c10::cuda::CUDAGuard guard(d.device());
+    torch::Tensor out = torch::empty({C, H, W, 3}, d.options().dtype(torch::kByte));
+    const int32_t stride = (int32_t)d.size(3);
+    gssdf_render_depth_normal_args a{};
+    a.C = (int32_t)C, a.W = (int32_t)W, a.H = (int32_t)H;
+    a.viewmats = vm.data_ptr<float>(), a.Ks = K.data_ptr<float>();
+    a.depth = d.data_ptr<float>() + (stride - 1), a.depth_stride = stride;
+    a.render_alphas = al.data_ptr<float>(), a.normal = out.data_ptr<uint8_t>();
+    check(gssdf_render_depth_normal_u8(&a, reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream())));
     return out;
 }

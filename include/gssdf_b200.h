@@ -1466,6 +1466,29 @@ typedef struct gssdf_render_frames_args {
 size_t gssdf_render_frames_workspace_bytes(int32_t C, int32_t W, int32_t H);
 int gssdf_render_frames_u8(const gssdf_render_frames_args *a, gssdf_stream_t stream);
 
+/* The depth-to-normal frame of export_test_image (include/neural_mapping/neural_mapping.cpp:1288-1310), the visual check on the
+   normal-consistency term: utils::tensor_to_cv_mat(sensor::depth_to_normal(depth) * alpha * 0.5f + 0.5f) of C views, with the depth
+   k_depth_type selects (0: the expected depth, channel 3 of out_colors, depth_stride 4; otherwise render_median, depth_stride 1).
+     n     = normalize(cross(P[y+1,x] - P[y-1,x], P[y,x+1] - P[y,x-1])) on interior pixels (F::normalize: c / max(|c|, 1e-12)), 0 on
+             the border rows and columns; P = the world point of the pixel centre (+0.5) at the depth, without the camera position
+             (it cancels in the differences). The stencil is gssdf_normal_consistency_loss's (one device helper).
+     frame = trunc8(fl_rn(fl_rn(n * alpha) * 0.5) + 0.5)        (trunc8 as for gssdf_render_frames_u8), RGB
+   The reference builds P with an fp32 ATen matmul whose summation order cuBLAS chooses, so its bytes are not pinned down: every byte is
+   within 1 of an fp64 evaluation of the same composition, and differs from it only where the pre-quantisation value lies within the
+   fp32 composition's own deviation from fp64 of a 1/255 step. Bit-identical from run to run and between one call of C views and C calls
+   of one view. No workspace, no allocation, no host sync. GSSDF_EINVAL before any launch for C outside [0, 65535], W or H < 1,
+   W H > 2^29, H > 524280, a NULL pointer, depth_stride < 1 or a float input that is not 4-byte aligned. C == 0 is a no-op. */
+typedef struct gssdf_render_depth_normal_args {
+    int32_t C, W, H;
+    const float *viewmats;        /* [C,4,4] world->camera */
+    const float *Ks;              /* [C,3,3] */
+    const float *depth;           /* [C,H,W,*] read at depth[pix * depth_stride] */
+    int32_t depth_stride;
+    const float *render_alphas;   /* [C,H,W,1] */
+    uint8_t *normal;              /* [C,H,W,3] overwritten */
+} gssdf_render_depth_normal_args;
+int gssdf_render_depth_normal_u8(const gssdf_render_depth_normal_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,7 +19,10 @@ the defaults and one with bck_color=1 and a mask (a quarter of the frame masked 
 so the splat count stays put) in alternating windows of --window iterations; prints the median and the spread (min, max) of the ms per
 iteration of each.
 
-  python tools/gs_train_bench.py [--sh 0,3] [--iters 4000] [--frames 60] [--window 50] [--rounds 4] [--options]
+--depth-type times the normal-consistency term on the median depth against the expected depth the same way: two trainers with
+depth_type 0 and 1, alternating windows of joint iterations after the normal term has switched on (iteration > 3000).
+
+  python tools/gs_train_bench.py [--sh 0,3] [--iters 4000] [--frames 60] [--window 50] [--rounds 4] [--options | --depth-type]
 """
 import argparse
 import json
@@ -86,6 +89,7 @@ def main():
     ap.add_argument("--window", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=4)
     ap.add_argument("--options", action="store_true", help="time bck_color=1 + a mask against the defaults")
+    ap.add_argument("--depth-type", action="store_true", help="time depth_type=1 (median depth) against depth_type=0")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     pack = S.box_room_pack(dev, 120, ds_pt_num=2000, seed=0)  # the depth pack of the GPU tests (its resolution does not enter the render)
@@ -116,18 +120,22 @@ def main():
                             sh_degree=sh, outlier_remove=True, **kw), n0
 
     w, half = args.window, args.iters // 2
-    if args.options:
+    if args.options or args.depth_type:
         mask = torch.ones(H, W, dtype=torch.bool, device=dev)
         mask[H // 4:3 * H // 4, W // 4:3 * W // 4] = False
+        start = max(half, 3001) if args.depth_type else half  # refine_gs_struct_start_iter 3000: the normal term is on from 3001
         for sh in [int(s) for s in args.sh.split(",")]:
-            runs = dict(defaults=trainer(sh)[0], bck_color_1_mask=trainer(sh, bck_color=1, mask=mask)[0])
+            if args.depth_type:
+                runs = dict(depth_type_0=trainer(sh, depth_type=0)[0], depth_type_1=trainer(sh, depth_type=1)[0])
+            else:
+                runs = dict(defaults=trainer(sh)[0], bck_color_1_mask=trainer(sh, bck_color=1, mask=mask)[0])
             for G in runs.values():
                 G.run_color_init()
                 G.start_rates()
             ms = {k: [] for k in runs}
             for r in range(2 * args.rounds + 1):
                 for k, G in runs.items():
-                    i0 = half + r * w
+                    i0 = start + r * w
                     t = ev_ms(lambda G=G, i0=i0: [G.step(j) for j in range(i0, min(i0 + w, args.iters))]) / w
                     if r > 0:  # the first window of each is the warm-up
                         ms[k].append(t)

@@ -2,6 +2,7 @@
 
 An eval set of Replica shape: 1200x680, SH degree 3, N = 200k and 1M splats of the box scene, V views. Two legs alternate in one run:
   render_views   batches of up to 8 views, the 8-bit colour, depth-colourmap and normal frames made on the device (9 bytes a pixel back)
+  render_views_depth2normal  the same with the depth-to-normal frame of the median depth as well (depth_normal=1, 12 bytes a pixel)
   reference      one view per render (a one-view SplatRenderer), the float colour, depth and normal pulled back with .cpu(), then
                  tensor_to_cv_mat / apply_colormap_to_depth's host conversions with cv2 (NeuralSLAM::render_path, utils.cpp:250-283)
 Both legs end with every frame in host memory; a leg's time is a host clock around the whole set, after a warm-up. Reports frames/s per
@@ -94,7 +95,8 @@ def main():
     for N in (int(s) for s in a.sizes.split(",")):
         sp = _splats(N, dev)
         R1 = RD.SplatRenderer(N, (DEG + 1) ** 2, 1, W, H, dev, 64 * N, sh_degree=DEG)
-        legs = {"render_views": lambda: list(VW.render_views(sp, poses, (W, H, K), sh_degree=DEG, batch=8))}
+        legs = {"render_views": lambda: list(VW.render_views(sp, poses, (W, H, K), sh_degree=DEG, batch=8)),
+                "render_views_depth2normal": lambda: list(VW.render_views(sp, poses, (W, H, K), sh_degree=DEG, batch=8, depth_normal=1))}
         if cv2 is not None:
             legs["reference"] = lambda: reference_leg(sp, poses, K, cv2, R1)
         for f in legs.values():  # warm-up: every shape of the timed window
