@@ -9,7 +9,7 @@
 
 namespace gssdf {
 
-__global__ void __launch_bounds__(256) densify_update_kernel(const gssdf_densify_update_args a) {
+__global__ void __launch_bounds__(256) densify_update_kernel(const gssdf_densify_update_args a, const float image_size) {
     const int j = blockIdx.x * 256 + threadIdx.x;
     const int nnz = min(a.counts->nnz, a.cap);
     if (j >= nnz) return;
@@ -21,8 +21,7 @@ __global__ void __launch_bounds__(256) densify_update_kernel(const gssdf_densify
     atomicAdd(a.count + g, 1.f);
     // visibilities and radii are >= 0: the float max is an integer max on the bit patterns
     atomicMax(reinterpret_cast<int *>(a.vis + g), __float_as_int(fmaxf(a.visibilities[j], 0.f)));
-    if (a.radii_state && a.radii) {
-        const float image_size = (float)max(a.width, a.height);
+    if (a.radii_state && a.radii) {  // image_size: max(width, height) of this call, or the caller's pinned normaliser
         const float r = (float)max(a.radii[2 * j], a.radii[2 * j + 1]) / image_size;
         atomicMax(reinterpret_cast<int *>(a.radii_state + g), __float_as_int(fmaxf(r, 0.f)));
     }
@@ -100,15 +99,26 @@ __global__ void __launch_bounds__(256) densify_remap_kernel(const gssdf_densify_
 
 using namespace gssdf;
 
-extern "C" int gssdf_densify_update_state(const gssdf_densify_update_args *a, gssdf_stream_t stream) {
-    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "densify_update_state: null args");
+static int densify_update_launch(const gssdf_densify_update_args *a, float image_size, gssdf_stream_t stream) {
     GSSDF_REQUIRE(a->N >= 0 && a->cap >= 0, GSSDF_EINVAL, "densify_update_state: negative size");
     if (a->N == 0 || a->cap == 0) return GSSDF_OK;
     GSSDF_REQUIRE(a->counts && a->gaussian_ids && a->v_densify && a->visibilities && a->grad2d && a->count && a->vis, GSSDF_EINVAL,
                   "densify_update_state: null pointer");
-    densify_update_kernel<<<cdiv(a->cap, 256), 256, 0, (cudaStream_t)stream>>>(*a);
+    densify_update_kernel<<<cdiv(a->cap, 256), 256, 0, (cudaStream_t)stream>>>(*a, image_size);
     GSSDF_LAUNCH_OK("densify_update_kernel");
     return GSSDF_OK;
+}
+
+extern "C" int gssdf_densify_update_state(const gssdf_densify_update_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "densify_update_state: null args");
+    return densify_update_launch(a, (float)max(a->width, a->height), stream);
+}
+
+extern "C" int gssdf_densify_update_state_sized(const gssdf_densify_update_args *a, float image_size, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "densify_update_state_sized: null args");
+    GSSDF_REQUIRE(!(a->radii_state && a->radii) || image_size > 0.f, GSSDF_EINVAL,
+                  "densify_update_state_sized: image_size must be positive, got %g", (double)image_size);
+    return densify_update_launch(a, image_size, stream);
 }
 
 extern "C" int gssdf_densify_flags(const gssdf_densify_flags_args *a, gssdf_stream_t stream) {

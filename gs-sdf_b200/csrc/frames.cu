@@ -10,6 +10,9 @@
 //
 // The depth-to-normal frame of export_test_image (include/neural_mapping/neural_mapping.cpp:1288-1310) is one more launch of its own
 // (gssdf_render_depth_normal_u8): it reads a 3x3 neighbourhood of the depth, so it tiles the image as the normal-consistency loss does.
+//
+// The other direction, for training (DESIGN 7q): gssdf_frames_u8_expand turns one 8-bit RGB training frame into the loss kernels' float
+// ground truth, the reference's convertTo(CV_32FC3, 1.0f / 255.0f), so that a dataset's frames can stay 8-bit until their iteration.
 #include <cmath>
 
 #include "common.cuh"
@@ -240,6 +243,15 @@ bool size_ok(int32_t C, int32_t W, int32_t H) {
 
 bool aligned(const void *p, uintptr_t a) { return ((uintptr_t)p & (a - 1)) == 0; }
 
+// one pixel per thread: three byte loads (the frame's RGB rows carry no alignment), one 16-byte store of the loss kernels' RGB + depth
+__global__ void __launch_bounds__(kThreads) frames_u8_expand_kernel(const uint8_t *__restrict__ src, int64_t HW, float4 *__restrict__ gt) {
+    const int64_t p = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    if (p >= HW) return;
+    constexpr float kInv255 = 1.0f / 255.0f;  // convertTo's alpha, rounded to fp32 once
+    const uint8_t *s = src + 3 * p;
+    gt[p] = make_float4(__fmul_rn((float)s[0], kInv255), __fmul_rn((float)s[1], kInv255), __fmul_rn((float)s[2], kInv255), 0.f);
+}
+
 }  // namespace
 }  // namespace gssdf
 
@@ -287,5 +299,18 @@ extern "C" int gssdf_render_depth_normal_u8(const gssdf_render_depth_normal_args
     const dim3 grid(cdiv(a->W, kDnX), cdiv(a->H, kDnY), a->C), block(kDnX, kDnY);
     depth_normal_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(*a);
     GSSDF_LAUNCH_OK("depth_normal_kernel");
+    return GSSDF_OK;
+}
+
+extern "C" int gssdf_frames_u8_expand(const gssdf_frames_u8_expand_args *a, gssdf_stream_t stream) {
+    GSSDF_REQUIRE(a != nullptr, GSSDF_EINVAL, "frames_u8_expand: null args");
+    GSSDF_REQUIRE(size_ok(1, a->W, a->H), GSSDF_EINVAL, "frames_u8_expand: bad frame %d x %d", a->W, a->H);
+    GSSDF_REQUIRE(a->offset >= 0, GSSDF_EINVAL, "frames_u8_expand: negative offset %lld", (long long)a->offset);
+    GSSDF_REQUIRE(a->store && a->gt, GSSDF_EINVAL, "frames_u8_expand: null pointer");
+    GSSDF_REQUIRE(aligned(a->gt, 16), GSSDF_EINVAL, "frames_u8_expand: gt must be 16-byte aligned");
+    const int64_t HW = (int64_t)a->W * a->H;
+    frames_u8_expand_kernel<<<cdiv(HW, (int64_t)kThreads), kThreads, 0, (cudaStream_t)stream>>>(a->store + a->offset, HW,
+                                                                                                 reinterpret_cast<float4 *>(a->gt));
+    GSSDF_LAUNCH_OK("frames_u8_expand_kernel");
     return GSSDF_OK;
 }

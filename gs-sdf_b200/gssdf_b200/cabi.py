@@ -215,6 +215,18 @@ def l1_loss_masked(Cn, W, H, out_colors, gt, w_rgb, w_depth, loss_out, v_out_col
     check(lib().gssdf_l1_loss_masked(_lib.C.byref(a), _stream()))
 
 
+def frames_u8_expand(store, offset, W, H, gt):
+    """gt [H,W,4] (float32, contiguous) <- frame of W x H interleaved RGB bytes at byte `offset` of the uint8 CUDA tensor `store`, as
+    x * (1.0f / 255.0f) in fp32; channel 3 <- 0 (gssdf_frames_u8_expand)."""
+    _req(store, torch.uint8, "store")
+    _req(gt, torch.float32, "gt")
+    if offset < 0 or offset + 3 * W * H > store.numel() or gt.numel() < 4 * W * H:
+        raise ValueError(f"gssdf_b200: a {W}x{H} frame at byte {offset} does not fit a store of {store.numel()} bytes and a gt of "
+                         f"{gt.numel()} floats")
+    a = make_args("gssdf_frames_u8_expand_args", store=store, offset=int(offset), W=W, H=H, gt=gt)
+    check(lib().gssdf_frames_u8_expand(_lib.C.byref(a), _stream()))
+
+
 # ---- SDF branch -------------------------------------------------------------------------------
 def sdf_net(table_half, mlp, n_levels=16, n_features=2, log2_hashmap_size=19, base_resolution=32, per_level_scale=2.0,
             hidden_dim=64, n_hidden=3, origin=(0.0, 0.0, 0.0), inv_size=0.0, mlp_mode=0, mlp_packed=None):
@@ -504,10 +516,16 @@ def scatter_rows3(n, index, n_gate, src, dst, n_live=None):
     check(lib().gssdf_scatter_rows3(_lib.C.byref(a), _stream()))
 
 
-def densify_update_state(N, cap, counts, gaussian_ids, v_densify, visibilities, radii, width, height, n_cameras, grad2d, count, vis, radii_state=None):
+def densify_update_state(N, cap, counts, gaussian_ids, v_densify, visibilities, radii, width, height, n_cameras, grad2d, count, vis, radii_state=None,
+                         image_size=None):
+    """image_size: the radii normaliser (gssdf_densify_update_state_sized); None: max(width, height) of this call
+    (gssdf_densify_update_state). grad2d scales by this call's width and height either way."""
     a = make_args("gssdf_densify_update_args", N=N, cap=cap, counts=counts, gaussian_ids=gaussian_ids, v_densify=v_densify, visibilities=visibilities,
                   radii=radii, width=width, height=height, n_cameras=n_cameras, grad2d=grad2d, count=count, vis=vis, radii_state=radii_state)
-    check(lib().gssdf_densify_update_state(_lib.C.byref(a), _stream()))
+    if image_size is None:
+        check(lib().gssdf_densify_update_state(_lib.C.byref(a), _stream()))
+    else:
+        check(lib().gssdf_densify_update_state_sized(_lib.C.byref(a), _lib.C.c_float(image_size), _stream()))
 
 
 def densify_flags(N, offsets, quats, scaling, opacity, flags, grad2d=None, count=None, vis=None, radii_state=None, grow_grad2d=0.0, grow_scale3d=0.0,

@@ -37,14 +37,22 @@ class Densifier:
         self.lr_end = lr_end
         self.gen = generator or torch.Generator(self.dev).manual_seed(0)
         self.log = []
+        # frames of several sizes (gstrain.GsTrainer with a camera per frame): the radii normaliser is max(W, H) of the first update,
+        # as the reference's `static image_size` (:658); grad2d keeps each frame's own scaling. False: every update normalises by its own
+        # frame, which is the same value when there is one size.
+        self.pin_image_size = False
+        self.image_size = None
 
     # ---- every iteration --------------------------------------------------------------------------------------------------------
     def update_state(self):
         """NeuralGS::update_state (:626-680) from the renderer's buffers of the step that just ran; no host sync."""
         R = self.T.R
+        if self.pin_image_size and self.image_size is None:
+            self.image_size = float(max(R.W, R.H))
         cabi.densify_update_state(self.T.N_live, R.cap, R.counts, R.p["gaussian_ids"], R.g["v_densify"], R.r["visibilities"],
                                   R.p["radii"] if self.scale2d_stop > 0 else None, R.W, R.H, R.C, self.state["grad2d"], self.state["count"],
-                                  self.state["vis"], self.state["radii"] if self.scale2d_stop > 0 else None)
+                                  self.state["vis"], self.state["radii"] if self.scale2d_stop > 0 else None,
+                                  image_size=self.image_size if self.pin_image_size else None)
 
     # ---- surgery ----------------------------------------------------------------------------------------------------------------
     def _flags(self, with_grow, it):

@@ -66,6 +66,62 @@ def outlier_due(i, interval):
     return i > 0 and i % interval == 0
 
 
+class FramesU8:
+    """8-bit RGB training frames of any sizes packed in one uint8 buffer (DESIGN 7q): frame i is sizes[i] = (W_i, H_i), W_i H_i 3 bytes of
+    interleaved RGB at byte offsets[i]. `data` lives on the device or in pinned host memory; GsTrainer expands one frame per iteration
+    on the device into the loss's float ground truth as the reference's convertTo(CV_32FC3, 1.0f / 255.0f) does (gssdf_frames_u8_expand),
+    after copying only that frame's bytes when the store is pinned. A quarter of the bytes of float frames."""
+
+    def __init__(self, data, sizes):
+        self.sizes = [(int(w), int(h)) for w, h in sizes]
+        if not self.sizes or min(min(wh) for wh in self.sizes) < 1:
+            raise ValueError("FramesU8: at least one frame, every width and height >= 1")
+        if not (isinstance(data, torch.Tensor) and data.dtype == torch.uint8 and data.dim() == 1 and data.is_contiguous()):
+            raise ValueError("FramesU8: data must be a contiguous uint8 tensor [n_bytes]")
+        self.offsets = np.concatenate([[0], np.cumsum([3 * w * h for w, h in self.sizes])]).astype(np.int64).tolist()
+        if data.numel() != self.offsets[-1]:
+            raise ValueError(f"FramesU8: {len(self.sizes)} frames need {self.offsets[-1]} bytes, data has {data.numel()}")
+        self.data = data
+
+    @classmethod
+    def pack(cls, frames, device=None, pin=False):
+        """frames: uint8 [H_i,W_i,3] RGB arrays or tensors. The store goes to `device`, or to pinned host memory with pin=True."""
+        ts = [torch.as_tensor(np.ascontiguousarray(f) if isinstance(f, np.ndarray) else f) for f in frames]
+        for t in ts:
+            if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[-1] != 3:
+                raise ValueError("FramesU8.pack: every frame must be uint8 [H,W,3]")
+        data = torch.cat([t.reshape(-1).cpu() for t in ts]) if ts else torch.zeros(0, dtype=torch.uint8)
+        data = data.pin_memory() if pin else data.to(device) if device is not None else data
+        return cls(data, [(int(t.shape[1]), int(t.shape[0])) for t in ts])
+
+    @property
+    def is_cuda(self):
+        return self.data.is_cuda
+
+    def frame(self, i):
+        """Frame i as uint8 [H,W,3] (a view of the store)."""
+        w, h = self.sizes[i]
+        return self.data[self.offsets[i]:self.offsets[i + 1]].view(h, w, 3)
+
+
+def parse_frames(images):
+    """GsTrainer's `images`: ("stack", [(W,H)] * T) for a float32 [T,H,W,3] tensor (the path of one camera), ("list", sizes) for a list
+    of float32 [H_i,W_i,3] tensors, ("u8", sizes) for a FramesU8 store. Shapes only: where the frames live is checked later."""
+    if isinstance(images, FramesU8):
+        return "u8", list(images.sizes)
+    if isinstance(images, (list, tuple)):
+        if not images:
+            raise ValueError("GsTrainer: the list of frames is empty")
+        for t in images:
+            if not (isinstance(t, torch.Tensor) and t.dtype == torch.float32 and t.dim() == 3 and t.shape[-1] == 3 and t.shape[0] >= 1
+                    and t.shape[1] >= 1):
+                raise ValueError("GsTrainer: every frame of a list must be a float32 tensor [H,W,3]")
+        return "list", [(int(t.shape[1]), int(t.shape[0])) for t in images]
+    if not (isinstance(images, torch.Tensor) and images.dtype == torch.float32 and images.dim() == 4 and images.shape[-1] == 3):
+        raise ValueError("GsTrainer: images must be a float32 tensor [T,H,W,3], a list of float32 [H,W,3] tensors or a FramesU8 store")
+    return "stack", [(int(images.shape[2]), int(images.shape[1]))] * int(images.shape[0])
+
+
 class GsTrainer:
     """gs_train on the device. `run()` runs colour initialisation (when enabled) and the gs_iter_step joint iterations; `histories()` reads
     the per-iteration device records once; `state()` returns what mesh.meshing, io.export_gs_to_ply and metrics.eval_render take.
@@ -73,15 +129,19 @@ class GsTrainer:
     sdf: an nsdf.SdfTrainer that has finished its stage (its state moves here; do not step it afterwards).
     splats: the dict gs_init.neural_gs_init / neural_gs_init_points return (anchors, offsets, quaternion, scaling, opacity, features_dc,
         features_rest), CUDA float32; capacity: the row capacity densification may grow to (rounded up to a multiple of 4).
-    poses: [T,4,4] camera-to-world (OpenCV axes); K: [3,3] pinhole; images: float32 [T,H,W,3] in [0,1], on the device or in pinned host
-        memory (then one frame is copied per iteration, asynchronously).
+    poses: [T,4,4] camera-to-world (OpenCV axes); K: [3,3] pinhole shared by every frame, or [T,3,3] a camera per frame (DESIGN 7q);
+        images: float32 [T,H,W,3] in [0,1], a list of T float32 [H_i,W_i,3] (frames of several sizes), or a FramesU8 store of 8-bit
+        frames expanded on the device; on the device or in pinned host memory (then one frame is copied per iteration, asynchronously).
+        Each frame is rendered at its own size with its own K (projection, normal term, background); the densifier's radii normaliser
+        is the first trained frame's max(W, H), as in the reference. The reference resizes every ground-truth frame to its first
+        camera's size, so it trains cameras of one size only; several sizes are an extension here, and nothing is resized.
     spatial_scale: 0.5 * inner_map_size. The remaining keywords are config/base.yaml's keys with its defaults; `densify` holds Densifier's
     keywords (prune_opa .. sh_degree_interval; sh_degree and sh_degree_interval are passed through from here).
     bck_color: the scene's k_bck_color, the background every render composites (colour initialisation, joint iterations, render()):
         0 black, 1 white (FAST-LIVO2, Oxford Spires, HKU), 2 a uniform random image drawn before every render from a device generator of
         its own (`bg_gen`, seeded from `seed`; the splat samples' draws stay those of modes 0 and 1).
     mask: the dataset's image mask, bool or uint8 [H,W], [H,W,1] or [H,W,3] on the device (nonzero = keep), applied to every frame's L1
-        and DSSIM terms as loss::rgb_loss / dssim_loss do.
+        and DSSIM terms as loss::rgb_loss / dssim_loss do; the reference has one mask, so every frame must then have its size.
     depth_type: the config's `depth_type` (k_depth_type), the depth the normal-consistency term differentiates from iteration
         refine_gs_struct_start_iter on: 0 the expected depth, any other int the rasteriser's median depth (bounded scenes; the COLMAP
         configurations set 1 or 3)."""
@@ -94,21 +154,30 @@ class GsTrainer:
         dev = sdf.dev
         if not (gs_iter_step >= 1 and outlier_removal_interval >= 1 and sh_degree_interval >= 1):
             raise ValueError("GsTrainer: gs_iter_step, outlier_removal_interval and sh_degree_interval must be >= 1")
-        hw = tuple(images.shape[1:3]) if isinstance(images, torch.Tensor) and images.dim() == 4 else (None, None)
+        is_4d = isinstance(images, torch.Tensor) and images.dim() == 4
+        kind, sizes = parse_frames(images) if not is_4d or images.shape[-1] == 3 else (None, [])
+        K_shape = tuple(torch.as_tensor(K).shape)
+        if kind is not None and K_shape not in ((3, 3), (len(sizes), 3, 3)):
+            raise ValueError(f"GsTrainer: K must be [3,3] or [T,3,3] with T = {len(sizes)} frames, got {K_shape}")
+        if mask is not None and len(set(sizes)) > 1:
+            raise ValueError("GsTrainer: an image mask needs every frame at its size, and the frames have several sizes")
+        hw = tuple(images.shape[1:3]) if is_4d else (sizes[0][1], sizes[0][0]) if sizes else (None, None)
         RD.check_photometric("GsTrainer", bck_color, mask, hw[0], hw[1], dev)
         RD.check_depth_type("GsTrainer", depth_type)
         for k in ("xyz", "origin", "direction", "depth"):
             if not sdf.pack[k].is_cuda:
                 raise ValueError(f"GsTrainer: the SdfTrainer's pack[{k!r}] must be on the device")
-        if not (isinstance(images, torch.Tensor) and images.dtype == torch.float32 and images.dim() == 4 and images.shape[-1] == 3):
-            raise ValueError("GsTrainer: images must be a float32 tensor [T,H,W,3]")
-        if not (images.is_cuda or images.is_pinned()):
-            raise ValueError("GsTrainer: images must be on the device or in pinned host memory")
-        n_frames, H, W = int(images.shape[0]), int(images.shape[1]), int(images.shape[2])
+        if kind is None:
+            parse_frames(images)  # raises: a 4-D tensor that is not [T,H,W,3]
+        store = images.data if kind == "u8" else images
+        for t in (store if kind == "list" else [store]):
+            if not (t.is_cuda or t.is_pinned()):
+                raise ValueError("GsTrainer: images must be on the device or in pinned host memory")
+        n_frames = len(sizes)
+        W, H = sizes[0]
         poses = torch.as_tensor(poses)
-        if n_frames < 1 or tuple(poses.shape) != (n_frames, 4, 4) or tuple(torch.as_tensor(K).shape) != (3, 3):
-            raise ValueError(f"GsTrainer: poses must be [{n_frames},4,4] and K [3,3] for {n_frames} images, got {tuple(poses.shape)} and "
-                             f"{tuple(torch.as_tensor(K).shape)}")
+        if n_frames < 1 or tuple(poses.shape) != (n_frames, 4, 4):
+            raise ValueError(f"GsTrainer: poses must be [{n_frames},4,4] for {n_frames} images, got {tuple(poses.shape)}")
         n0 = int(splats["anchors"].shape[0])
         if not 1 <= n0 <= capacity:
             raise ValueError(f"GsTrainer: {n0} initial splats do not fit a capacity of {capacity}")
@@ -119,8 +188,13 @@ class GsTrainer:
         self.outlier_remove, self.outlier_dist, self.outlier_interval = bool(outlier_remove), float(outlier_dist), int(outlier_removal_interval)
         self.spatial_scale = float(spatial_scale)
         self.viewmats = torch.linalg.inv(poses.to(torch.float64)).to(torch.float32).to(dev).contiguous()
-        self.Ks = torch.as_tensor(K, dtype=torch.float32).reshape(1, 3, 3).to(dev).contiguous()
-        self.images = images
+        Kt = torch.as_tensor(K, dtype=torch.float32)
+        self.Ks = Kt.reshape(-1, 3, 3)[:1].to(dev).contiguous()  # frame 0's camera (every frame's with K [3,3])
+        self.K_frames = Kt.reshape(n_frames, 1, 3, 3).to(dev).contiguous() if Kt.dim() == 3 else None
+        self.K_cur = self.Ks
+        self.images, self.frames_kind, self.sizes = images, kind, sizes
+        distinct = sorted(set(sizes))
+        self.multi_size = len(distinct) > 1
         K_sh = (sh_degree + 1) ** 2
         net = sdf.net_mod
         cap = (int(capacity) + 3) // 4 * 4  # a multiple of 4 rows: every segment of the flat buffers starts 16-byte aligned
@@ -129,7 +203,7 @@ class GsTrainer:
                                      visible_thr=visible_thr, mlp_mode=1, eikonal_mode=1, align_weight=sdf.align_w, rgb_weight=rgb_weight,
                                      dssim_weight=dssim_weight, depth_weight=0.0, normal_weight=0.0, isotropic_weight=isotropic_weight,
                                      spatial_scale=self.spatial_scale, n_live=n0, delta_dev=sdf.std_dev, bck_color=bck_color, mask=mask,
-                                     depth_type=depth_type)
+                                     depth_type=depth_type, frame_sizes=distinct if self.multi_size else None)
         T.origin, T.inv_size, T.bce_isigma = net.origin, net.inv_size, sdf.bce_isigma
         T.set_octree(sdf.rs.tree)
         n_sdf = sdf.n_table + sdf.n_mlp
@@ -142,14 +216,21 @@ class GsTrainer:
         dkw = dict(densify or {})
         dkw.update(sh_degree=sh_degree, sh_degree_interval=sh_degree_interval)
         self.D = DN.Densifier(T, n_frames, spatial_scale=self.spatial_scale, lr_end=sdf.lr_end, **dkw)
+        self.D.pin_image_size = self.multi_size
         self.sdf_steps0 = sdf.t
         self.cpu_gen = torch.Generator().manual_seed(seed)
         self.gen = torch.Generator(dev).manual_seed(seed)
         self.bg_gen = torch.Generator(dev).manual_seed(seed + (1 << 32))  # bck_color 2's backgrounds: not the randns stream
         self.randns = torch.empty(T.R.cap, 2, dtype=torch.float32, device=dev)  # the splat samples' draw, fresh every render
         self.perm = None
-        self.gt = torch.zeros(1, H, W, 4, dtype=torch.float32, device=dev)  # RGB + the (unused) depth channel the loss kernels read
-        self.stage = None if images.is_cuda else torch.empty(H, W, 3, dtype=torch.float32, device=dev)
+        # RGB + the (unused) depth channel the loss kernels read, viewed at the current frame's size
+        self._gt_store = torch.zeros(4 * T.R.max_pixels, dtype=torch.float32, device=dev)
+        self.gt = self._gt_store[:4 * H * W].view(1, H, W, 4)
+        pinned = [t for t in (images if kind == "list" else [store]) if not t.is_cuda]
+        # staging for pinned frames: one frame's floats, or one frame's bytes of an 8-bit store
+        self._stage_store = (None if not pinned else torch.empty(3 * T.R.max_pixels, dtype=torch.uint8 if kind == "u8" else torch.float32,
+                                                                  device=dev))
+        self.stage = self._stage_store[:3 * H * W].view(H, W, 3) if self._stage_store is not None and kind != "u8" else None
         f32, i32 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int32, device=dev)
         n_it = self.iters
         self.h_color = torch.zeros(n_frames if self.color_init else 0, **f32)
@@ -165,9 +246,30 @@ class GsTrainer:
             self.perm = torch.randperm(self.train_num, generator=self.cpu_gen).tolist()
         return self.perm[i % self.train_num]
 
+    def set_frame(self, W, H):
+        """Train at W x H from here on: the renderer, the background and the ground truth become views of that size."""
+        if (self.T.R.W, self.T.R.H) == (W, H) and tuple(self.gt.shape[1:3]) == (H, W):
+            return
+        self.T.set_frame(W, H)
+        self.gt = self._gt_store[:4 * H * W].view(1, H, W, 4)
+        if self._stage_store is not None and self.frames_kind != "u8":
+            self.stage = self._stage_store[:3 * H * W].view(H, W, 3)
+
     def load_frame(self, cam):
-        """gt <- images[cam] (the reference's get_image(..).to(k_device)); a pinned frame goes through the staging buffer asynchronously."""
-        if self.stage is None:
+        """gt <- images[cam] (the reference's get_image(..).to(k_device)) at the frame's size, with the frame's K in K_cur; a pinned frame
+        goes through the staging buffer asynchronously, an 8-bit frame is expanded on the device."""
+        W, H = self.sizes[cam]
+        self.set_frame(W, H)
+        self.K_cur = self.Ks if self.K_frames is None else self.K_frames[cam]
+        if self.frames_kind == "u8":
+            st = self.images
+            if st.is_cuda:
+                cabi.frames_u8_expand(st.data, st.offsets[cam], W, H, self.gt)
+            else:
+                stage = self._stage_store[:3 * W * H]
+                stage.copy_(st.data[st.offsets[cam]:st.offsets[cam + 1]], non_blocking=True)
+                cabi.frames_u8_expand(stage, 0, W, H, self.gt)
+        elif self.images[cam].is_cuda:
             self.gt[0, ..., :3].copy_(self.images[cam])
         else:
             self.stage.copy_(self.images[cam], non_blocking=True)
@@ -188,7 +290,7 @@ class GsTrainer:
         for i in range(self.train_num):
             vm = self.load_frame(self.camera(i))
             self.draw_background()
-            T.color_step(vm, self.Ks, self.gt)
+            T.color_step(vm, self.K_cur, self.gt)
             self.h_color[i:i + 1].copy_(T.R.loss)
         T.lr = [color_init_lr(lr) for lr in base]
         T.flat_grad[:T.t0].zero_()  # the structure's gradients of the frozen iterations are discarded
@@ -209,13 +311,13 @@ class GsTrainer:
         self.randns.normal_(generator=self.gen)  # the reference's randn of every render (Projection.cpp:728)
         self.draw_background()
         if self.detach:
-            loss, sdf_loss = T.train_step(vm, self.Ks, self.gt, None, None, self.randns)
+            loss, sdf_loss = T.train_step(vm, self.K_cur, self.gt, None, None, self.randns)
         else:
             S.draw()
             cabi.sdf_ray_batch(S.pack, S.rand, S.n_rays_dev, S.rays)
             rs.sample(S.rays["origin"], S.rays["direction"], S.rays["depth"], S.rays["xyz"], n_live=S.n_rays_dev, sample_std=S.std_dev)
             torch.bitwise_or(S.overflow, rs.counts[2:3], out=S.overflow)
-            loss, sdf_loss = T.train_step(vm, self.Ks, self.gt, rs.xyz, rs.ray_sdf, self.randns, ray_n_live=rs.counts)
+            loss, sdf_loss = T.train_step(vm, self.K_cur, self.gt, rs.xyz, rs.ray_sdf, self.randns, ray_n_live=rs.counts)
         T.adam_clocks(sdf=not self.detach)
         if self.detach:
             T.flat_grad[T.t0:].zero_()  # [C]'s SDF gradient has no optimiser group to consume it
@@ -257,7 +359,7 @@ class GsTrainer:
 
     def state(self):
         """dict(net=the SdfNet with the trained SDF written back (mesh.meshing), splats=the trained splats as io.export_gs_to_ply takes them
-        (anchors, offsets, features_dc, features_rest, opacity, scaling, quaternion), render(cam_index or viewmat) -> [H,W,3] image for
+        (anchors, offsets, features_dc, features_rest, opacity, scaling, quaternion), render(viewmat, camera=None) -> [H,W,3] image for
         metrics.eval_render)."""
         T = self.T
         p = T.params  # brings every SH row current
@@ -270,16 +372,23 @@ class GsTrainer:
                       opacity=sc["opacities"], scaling=sc["scales"], quaternion=sc["quats"])
         return dict(net=self.sdf.net_mod, splats=splats, render=self.render)
 
-    def render(self, viewmat):
+    def render(self, viewmat, camera=None):
         """The colour image [H,W,3] of a world->camera pose [4,4] at the current SH degree on the configured background (the render the
-        reference exports and scores; bck_color 2 draws a fresh background for it)."""
+        reference exports and scores; bck_color 2 draws a fresh background for it). camera: (W, H, K [3,3]), e.g. an entry of
+        io.load_colmap_cameras' table; None renders with frame 0's camera. Its pixel count and tile grid must fit the largest training
+        frame's (the renderer's storage)."""
         T = self.T
         T.flush_sh()
         vm = torch.as_tensor(viewmat, dtype=torch.float32).reshape(1, 4, 4).to(self.dev).contiguous()
+        if camera is None:
+            (W, H), K = self.sizes[0], self.Ks
+        else:
+            W, H, K = int(camera[0]), int(camera[1]), torch.as_tensor(camera[2], dtype=torch.float32).reshape(1, 3, 3).to(self.dev).contiguous()
+        T.view_frame(W, H)  # the image mask belongs to the loss, not to the render
         sc = T.scene
         raw = dict(sc["raw"], sh_catch_up=None)
         self.draw_background()
-        T.R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], vm, self.Ks, raw=raw, bck_color=T.bck_color, bg=T.bg)
+        T.R.forward(sc["means"], sc["quats"], sc["scales"], sc["opacities"], sc["sh"], vm, K, raw=raw, bck_color=T.bck_color, bg=T.bg)
         return T.R.out_colors[0, ..., :3].clone()
 
     def __repr__(self):

@@ -177,3 +177,38 @@ def read_mesh_ply(path):
     if nf and not (fr[:, 0] == 3).all():
         raise ValueError(f"{path}: only triangle faces are supported")
     return rec["xyz"].astype(np.float32), fr[:, 1:].astype(np.int32), rec["rgb"].astype(np.uint8)
+
+
+def load_colmap_cameras(path, scale=1.0):
+    """COLMAP's cameras.txt as DataParser::load_cameras reads it (include/data_loader/data_parsers/base_parser.cpp:429-496): the camera
+    table {camera_id: (W, H, K)} with K a float32 [3,3] pinhole, in the form views.render_views and gstrain.GsTrainer take. A line whose
+    first character is `#` is a comment; every other line is `camera_id model width height params...`. PINHOLE and OPENCV are read as
+    pinhole `fx fy cx cy` (OPENCV's distortion parameters are ignored, as the reference does). `scale` is the sensor's fp32 image scale:
+    width / height become (int)(scale * w) (fp32 product, truncated) and fx, fy, cx, cy the fp32 products with scale. A repeated id
+    keeps its last line. OPENCV_FISHEYE raises ValueError (undistortion is out of scope here), as does any other model, a missing file or
+    a line that does not parse. One departure: blank lines are skipped (the reference reads them as a camera and fails)."""
+    if not os.path.exists(path):
+        raise ValueError(f"Camera file does not exist: {path}")
+    s = np.float32(scale)
+    cams = {}
+    with open(path, "r", encoding="latin-1") as f:
+        for line in f.read().split("\n"):
+            if line.startswith("#") or not line.strip():
+                continue
+            tok = line.split()
+            model = tok[1] if len(tok) > 1 else ""
+            if model == "OPENCV_FISHEYE":
+                raise ValueError(f"load_colmap_cameras: OPENCV_FISHEYE needs undistortion, which is not supported: {line!r}")
+            if model not in ("PINHOLE", "OPENCV"):
+                raise ValueError(f"Unsupported camera model: {model}")
+            try:
+                cam_id, w, h = int(tok[0]), int(tok[2]), int(tok[3])
+                fx, fy, cx, cy = (np.float32(float(v)) for v in tok[4:8])
+                if len(tok) < 8:
+                    raise IndexError
+            except (ValueError, IndexError):
+                raise ValueError(f"load_colmap_cameras: cannot parse {line!r}") from None
+            W, H = int(s * np.float32(w)), int(s * np.float32(h))
+            fx, fy, cx, cy = (s * v for v in (fx, fy, cx, cy))
+            cams[cam_id] = (W, H, torch.tensor([[fx, 0.0, cx], [0.0, fy, cy], [0.0, 0.0, 1.0]], dtype=torch.float32))
+    return cams

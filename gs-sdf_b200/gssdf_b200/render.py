@@ -46,14 +46,37 @@ def expand_mask(mask, H, W):
     return None if mask is None else mask.reshape(H, W, -1).ne(0).to(torch.uint8).expand(H, W, 3).contiguous()
 
 
+def frame_maxima(sizes, tile_size=16):
+    """(largest pixel count, largest tile count) over a list of (W, H) frame sizes: what per-pixel and per-tile storage must hold."""
+    return (max(int(w) * int(h) for w, h in sizes),
+            max(math.ceil(int(w) / tile_size) * math.ceil(int(h) / tile_size) for w, h in sizes))
+
+
+# per-pixel buffers of SplatRenderer: (dict attribute or None, key, channels, dtype, zero-initialised)
+_PIXEL_BUFFERS = [("r", "render_colors", 3, torch.float32, False), ("r", "render_depths", 1, torch.float32, False),
+                  ("r", "render_alphas", 1, torch.float32, False), ("r", "render_normals", 3, torch.float32, False),
+                  ("r", "render_median", 1, torch.float32, False), ("r", "last_ids", None, torch.int32, False),
+                  ("r", "median_ids", None, torch.int32, False), (None, "out_colors", 4, torch.float32, False),
+                  (None, "out_normals", 3, torch.float32, False), (None, "v_out_colors", 4, torch.float32, False),
+                  (None, "v_out_normals", 3, torch.float32, True), ("v_r", "colors", 3, torch.float32, False),
+                  ("v_r", "depths", 1, torch.float32, False), ("v_r", "alphas", 1, torch.float32, False),
+                  ("v_r", "normals", 3, torch.float32, False), ("v_r", "median", 1, torch.float32, True)]
+
+
 class SplatRenderer:
-    def __init__(self, N, K, C, W, H, device, isect_cap, tile_size=16, near=0.05, far=300.0, sh_degree=3, presort_cull=True):
-        self.N, self.K, self.C, self.W, self.H, self.tile = N, K, C, W, H, tile_size
+    def __init__(self, N, K, C, W, H, device, isect_cap, tile_size=16, near=0.05, far=300.0, sh_degree=3, presort_cull=True,
+                 frame_sizes=None):
+        """frame_sizes: every (W, H) the renderer will be asked to render (DESIGN 7q). Per-pixel and per-tile storage is allocated for the
+        largest pixel count and the largest tile grid among them and `set_frame` re-views it as contiguous [C,H,W,.] buffers of one
+        size; the raster, tile and DSSIM workspaces are sized for the maxima. None: (W, H) only, today's exact allocation. The renderer
+        starts at (W, H)."""
+        self.N, self.K, self.C, self.tile = N, K, C, tile_size
         self.near, self.far, self.sh_degree = near, far, sh_degree
         self.dev = device
         self.cap = N * C
         self.isect_cap = int(isect_cap)
-        self.tw, self.th = math.ceil(W / tile_size), math.ceil(H / tile_size)
+        self.frame_sizes = [(int(W), int(H))] + [(int(w), int(h)) for w, h in (frame_sizes or [])]
+        self.max_pixels, self.max_tiles = frame_maxima(self.frame_sizes, tile_size)
         f32 = dict(dtype=torch.float32, device=device)
         i32 = dict(dtype=torch.int32, device=device)
         cap = self.cap
@@ -66,16 +89,17 @@ class SplatRenderer:
         self.presort_cull = bool(presort_cull) and tile_size == 16
         self.conics = e(cap, 8) if self.presort_cull else None
         self.flatten_ids = e(self.isect_cap, **i32)
-        self.offsets = e(C, self.th, self.tw, **i32)
+        # flat storage behind every per-pixel buffer and the tile offsets; set_frame views its leading C*H*W*channels elements.
         # no render_distort / render_Ts: the distortion loss is off in GS-SDF (distloss = false), the kernel then skips those terms
-        self.r = dict(render_colors=e(C, H, W, 3), render_depths=e(C, H, W, 1), render_alphas=e(C, H, W, 1),
-                      render_normals=e(C, H, W, 3), render_median=e(C, H, W, 1),
-                      last_ids=e(C, H, W, **i32), median_ids=e(C, H, W, **i32), visibilities=e(cap, 1))
-        self.out_colors, self.out_normals = e(C, H, W, 4), e(C, H, W, 3)
-        # cotangents
-        self.v_out_colors, self.v_out_normals = e(C, H, W, 4), torch.zeros(C, H, W, 3, **f32)
-        self.v_r = dict(colors=e(C, H, W, 3), depths=e(C, H, W, 1), alphas=e(C, H, W, 1), normals=e(C, H, W, 3),
-                        median=torch.zeros(C, H, W, 1, **f32))
+        self._pix = {}
+        for grp, key, ch, dt, zero in _PIXEL_BUFFERS:
+            n = C * self.max_pixels * (ch or 1)
+            self._pix[(grp, key)] = (torch.zeros if zero else torch.empty)(n, dtype=dt, device=device)
+        self._offsets_store = e(C * self.max_tiles, **i32)
+        self.r, self.v_r = {}, {}
+        self.W = self.H = None
+        self.set_frame(W, H)
+        self.r["visibilities"] = e(cap, 1)
         self.g = dict(v_means2d=None, v_ray_transforms=e(cap, 3, 3), v_colors=e(cap, 3), v_opacities=e(cap),
                       v_normals=e(cap, 3), v_densify=e(cap, 2))
         # flat gradient buffer: means[N,3] quats[N,4] scales[N,3] opacities[N] sh[N,K,3]
@@ -92,9 +116,40 @@ class SplatRenderer:
         # dedicated raster workspace (records, conics, culled lists | gradient records): the backward reuses the forward's part
         self.raster_ws = cabi.Workspace(device)
         self.loss_ws = cabi.Workspace(device)  # DSSIM derivative maps
-        self.raster_ws.get(cabi.lib().gssdf_raster2dgs_bwd_workspace_bytes(C, W, H, cap, cabi._lib.C.c_int64(self.isect_cap)))
+        L, i64 = cabi.lib(), cabi._lib.C.c_int64
+        self.raster_ws.get(max(L.gssdf_raster2dgs_bwd_workspace_bytes(C, w, h, cap, i64(self.isect_cap)) for w, h in self.frame_sizes))
+        if frame_sizes:  # several sizes: no workspace grows between frames
+            self.ws.get(max(max(L.gssdf_tile_encode_workspace_bytes(C, w, h, tile_size, i64(self.isect_cap)),
+                                L.gssdf_project2dgs_workspace_bytes(N, C)) for w, h in self.frame_sizes))
+            self.loss_ws.get(max(L.gssdf_dssim_workspace_bytes(C, w, h) for w, h in self.frame_sizes))
         self.prof_fwd = self.prof_bwd = None  # optional (start, stop) torch.cuda.Event pairs around the raster kernels
         self.stage_events = None  # profiling: list of (stage name, torch.cuda.Event recorded AFTER the stage) (bench.py per-stage table)
+
+    def set_frame(self, W, H):
+        """Render frames of W x H from here on: every per-pixel buffer (r, v_r, out_*, v_out_*) and the tile offsets become contiguous
+        [C,H,W,.] views of the leading elements of their storage. The size must fit the storage frame_sizes allocated; the pixels past a
+        smaller frame keep whatever a larger one left there, and no kernel reads them."""
+        W, H = int(W), int(H)
+        if (W, H) == (self.W, self.H):
+            return
+        tw, th = math.ceil(W / self.tile), math.ceil(H / self.tile)
+        if W < 1 or H < 1 or W * H > self.max_pixels or tw * th > self.max_tiles:
+            raise ValueError(f"SplatRenderer.set_frame: a {W}x{H} frame does not fit storage for {self.max_pixels} pixels and "
+                             f"{self.max_tiles} tiles (frame_sizes)")
+        C = self.C
+        self.W, self.H, self.tw, self.th = W, H, tw, th
+        for grp, key, ch, _, _ in _PIXEL_BUFFERS:
+            st = self._pix[(grp, key)]
+            v = st[:C * H * W * (ch or 1)].view((C, H, W, ch) if ch else (C, H, W))
+            if grp is None:
+                setattr(self, key, v)
+            else:
+                getattr(self, grp)[key] = v
+        self.offsets = self._offsets_store[:C * th * tw].view(C, th, tw)
+
+    def _zero_pixels(self, grp, key):
+        """Zero a buffer's whole storage (the tail a smaller frame does not view included)."""
+        self._pix[(grp, key)].zero_()
 
     def _mark(self, name):
         if self.stage_events is not None:
@@ -177,11 +232,11 @@ class SplatRenderer:
                                          w_normal, self.loss, v_depth=self.v_out_colors.data_ptr() + 12, v_depth_stride=4,
                                          v_out_normals=self.v_out_normals)
             self._v_normals_dirty = True
-        elif getattr(self, "_v_normals_dirty", False):
-            self.v_out_normals.zero_()
+        elif getattr(self, "_v_normals_dirty", False):  # the whole storage: a later, larger frame must read zeros too
+            self._zero_pixels(None, "v_out_normals")
             self._v_normals_dirty = False
         if not (w_normal > 0 and median_depth) and getattr(self, "_v_median_dirty", False):
-            self.v_r["median"].zero_()
+            self._zero_pixels("v_r", "median")
             self._v_median_dirty = False
         if w_isotropic > 0:  # isotropic regulariser on the visible splats' (x, y) scales (neural_mapping.cpp:268-276)
             cabi.isotropic_loss(self.N, cap, self.counts, self.p["gaussian_ids"], scales, raw is not None, w_isotropic, self.loss,
@@ -249,18 +304,20 @@ class GsSdfStep:
     def __init__(self, N, K, W, H, device, isect_cap, sdf_net_cfg, n_ray_samples=32768, sh_degree=3, origin=(0.0, 0.0, 0.0),
                  map_size=14.0, bce_sigma=0.1, delta=None, eikonal_weight=0.1, gs_sdf_weight=1e-3, visible_thr=0.1, mlp_mode=None,
                  eikonal_mode=None, align_weight=0.1, rgb_weight=0.8, dssim_weight=0.2, depth_weight=0.1, normal_weight=0.0,
-                 isotropic_weight=0.0, delta_dev=None, bck_color=0, mask=None, depth_type=0):
+                 isotropic_weight=0.0, delta_dev=None, bck_color=0, mask=None, depth_type=0, frame_sizes=None):
         """delta_dev: float32 CUDA tensor [1] read by every SDF call of [A] and [C] in place of the host scalar `delta` (the sample std the
         SDF stage adapts on the device, nsdf.SdfTrainer.std_dev); the ray-site forward then also evaluates the base variant into ray_y1.
         bck_color (k_bck_color: 0 black, 1 white, 2 random) and mask (bool / uint8 [H,W], [H,W,1] or [H,W,3] on the device, one for every
         frame): the render's background and the photometric loss's image mask (DESIGN 7o), in the joint step and in color_step. With
         bck_color 2 the render composites self.bg [1,H,W,3], which the caller fills before every render (gstrain.GsTrainer draws it).
-        depth_type (k_depth_type): the depth of the normal-consistency term, 0 the expected depth, any other int the median depth."""
+        depth_type (k_depth_type): the depth of the normal-consistency term, 0 the expected depth, any other int the median depth.
+        frame_sizes: the (W, H) of every frame the step will train or render (SplatRenderer; set_frame switches between them)."""
         check_photometric("GsSdfStep", bck_color, mask, H, W, device)
         self.median_depth = check_depth_type("GsSdfStep", depth_type)
-        self.R = SplatRenderer(N, K, 1, W, H, device, isect_cap, sh_degree=sh_degree)
+        self.R = SplatRenderer(N, K, 1, W, H, device, isect_cap, sh_degree=sh_degree, frame_sizes=frame_sizes)
         self.bck_color, self.mask = int(bck_color), expand_mask(mask, H, W)
-        self.bg = torch.zeros(1, H, W, 3, dtype=torch.float32, device=device) if self.bck_color == 2 else None
+        self._bg_store = torch.zeros(3 * self.R.max_pixels, dtype=torch.float32, device=device) if self.bck_color == 2 else None
+        self.bg = self._bg_store[:3 * H * W].view(1, H, W, 3) if self.bck_color == 2 else None
         self.dev, self.N, self.n_ray = device, N, n_ray_samples
         self.cfg = dict(sdf_net_cfg)
         self.origin, self.inv_size = tuple(origin), 1.0 / map_size
@@ -322,6 +379,24 @@ class GsSdfStep:
         self.sdf_stream_priority = 0
         self._side = None
         self._ev_fwd, self._ev_c = torch.cuda.Event(), torch.cuda.Event()
+
+    def set_frame(self, W, H, mask=None):
+        """Train / render W x H frames from here on (SplatRenderer.set_frame): the renderer's per-pixel buffers and the background
+        (bck_color 2, drawn by the caller after this) become views of that size. mask: a new image mask of that size (check_photometric);
+        without one, the current mask stays and must have that size."""
+        if mask is not None:
+            check_photometric("GsSdfStep.set_frame", self.bck_color, mask, int(H), int(W), self.dev)
+        elif self.mask is not None and tuple(self.mask.shape[:2]) != (int(H), int(W)):
+            raise ValueError(f"GsSdfStep.set_frame: the image mask is {tuple(self.mask.shape[:2])}, the frame {int(H)}x{int(W)} (H x W)")
+        self.view_frame(W, H)
+        if mask is not None:
+            self.mask = expand_mask(mask, self.R.H, self.R.W)
+
+    def view_frame(self, W, H):
+        """set_frame without the mask: for renders outside the loss."""
+        self.R.set_frame(W, H)
+        if self._bg_store is not None:
+            self.bg = self._bg_store[:3 * self.R.H * self.R.W].view(1, self.R.H, self.R.W, 3)
 
     @contextlib.contextmanager
     def sdf_stage(self):

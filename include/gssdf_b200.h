@@ -808,6 +808,12 @@ typedef struct gssdf_densify_update_args {
     float *radii_state;           /* [N] max= max(radii) / max(W, H), or NULL */
 } gssdf_densify_update_args;
 int gssdf_densify_update_state(const gssdf_densify_update_args *a, gssdf_stream_t stream);
+/* update_state with the radii normaliser given: radii_state max= max(radii) / image_size instead of / max(width, height). The
+   reference's normaliser is `static image_size = max(width, height)` (neural_gaussian.cpp:658), fixed at its first call, while
+   grad2d is scaled by the width and height of every call; a caller training frames of several sizes pins image_size at its first
+   update and passes each frame's width and height. GSSDF_EINVAL for image_size <= 0 or NaN when radii are tracked; otherwise the
+   arguments and the launch are gssdf_densify_update_state's. */
+int gssdf_densify_update_state_sized(const gssdf_densify_update_args *a, float image_size, gssdf_stream_t stream);
 
 /* Per-splat decision bits of grow_gs (:690-720), prune_gs (:842-876), prune_invisible_gs (:878-892), prune_nan_gs (:894-905). */
 enum { GSSDF_DENSIFY_DUPLI = 1, GSSDF_DENSIFY_SPLIT = 2, GSSDF_DENSIFY_PRUNE_OPA = 4, GSSDF_DENSIFY_PRUNE_SMALL = 8,
@@ -1488,6 +1494,22 @@ typedef struct gssdf_render_depth_normal_args {
     uint8_t *normal;              /* [C,H,W,3] overwritten */
 } gssdf_render_depth_normal_args;
 int gssdf_render_depth_normal_u8(const gssdf_render_depth_normal_args *a, gssdf_stream_t stream);
+
+/* One 8-bit training frame expanded into the ground-truth buffer the loss kernels read (gssdf_l1_loss's gt, DESIGN 7q): frame i of a
+   packed store of interleaved RGB uint8 frames lies at byte `offset` of `store` with its own width and height, and
+     gt[y, x, c] = fl_rn((float)store[offset + 3 (y W + x) + c] * (1.0f / 255.0f))   for c < 3,   gt[y, x, 3] = 0
+   -- the reference's cv_mat_to_tensor (convertTo(CV_32FC3, 1.0f / 255.0f) after the BGR -> RGB swap; base_parser.cpp:347-376), per
+   channel the fp32 product. gt is [H,W,4], contiguous, 16-byte aligned, overwritten (channel 3 is the depth the loss's depth term
+   reads; the joint stage weights it 0). The store may be device memory or a device copy of one frame (offset 0) that the caller
+   staged from pinned host memory on the same stream. No workspace, no allocation, no host sync. GSSDF_EINVAL before any launch for
+   W or H < 1, W H > 2^29, a negative offset, a NULL pointer or a misaligned gt. */
+typedef struct gssdf_frames_u8_expand_args {
+    const uint8_t *store;         /* packed RGB frames */
+    int64_t offset;               /* byte offset of the frame in store */
+    int32_t W, H;
+    float *gt;                    /* [H,W,4] */
+} gssdf_frames_u8_expand_args;
+int gssdf_frames_u8_expand(const gssdf_frames_u8_expand_args *a, gssdf_stream_t stream);
 
 #ifdef __cplusplus
 }
