@@ -227,6 +227,43 @@ def frames_u8_expand(store, offset, W, H, gt):
     check(lib().gssdf_frames_u8_expand(_lib.C.byref(a), _stream()))
 
 
+def undistort_map(K, D, new_K, model, W, H, out):
+    """out int16 [H,W,4] (CUDA, contiguous) <- the fixed-point undistortion map of one camera (gssdf_undistort_map). K, new_K: 3x3,
+    D: up to 5 coefficients (k1 k2 p1 p2 k3 for model 0, k1..k4 for model 1); all are passed as fp32."""
+    _req(out, torch.int16, "map")
+    if out.numel() < 4 * W * H:
+        raise ValueError(f"gssdf_b200: a map of {out.numel()} int16 is too small for {W}x{H}")
+    d = [float(v) for v in torch.as_tensor(D, dtype=torch.float32).reshape(-1).tolist()]
+    if len(d) > 5:
+        raise ValueError(f"gssdf_b200: {len(d)} distortion coefficients, at most 5")
+    f9 = lambda M: torch.as_tensor(M, dtype=torch.float32).reshape(-1).tolist()
+    a = make_args("gssdf_undistort_map_args", model=int(model), W=int(W), H=int(H), K=f9(K), D=d + [0.0] * (5 - len(d)), new_K=f9(new_K),
+                  map=out)
+    check(lib().gssdf_undistort_map(_lib.C.byref(a), _stream()))
+
+
+def undistort_u8(src, dst, offsets, sizes, map_ids, maps):
+    """dst <- src remapped frame by frame (gssdf_undistort_u8). src, dst: uint8 CUDA tensors of one size holding packed RGB frames;
+    offsets / sizes / map_ids: per-frame byte offsets, (W, H) and indices into `maps` (host sequences); maps: int16 [H,W,4] CUDA maps."""
+    _req(src, torch.uint8, "src")
+    _req(dst, torch.uint8, "dst")
+    if src.numel() != dst.numel():
+        raise ValueError(f"gssdf_b200: src has {src.numel()} bytes, dst {dst.numel()}")
+    for m in maps:
+        _req(m, torch.int16, "map")
+        if m.device != src.device or dst.device != src.device:
+            raise ValueError(f"gssdf_b200: src, dst and every map must be on one device ({src.device}, {dst.device}, {m.device})")
+    n, C = len(offsets), _lib.C
+    off = (C.c_int64 * max(n, 1))(*[int(o) for o in offsets])
+    sz = (C.c_int32 * max(2 * n, 1))(*[int(v) for wh in sizes for v in wh])
+    ids = (C.c_int32 * max(n, 1))(*[int(i) for i in map_ids])
+    mp = (C.c_void_p * max(len(maps), 1))(*[m.data_ptr() for m in maps])
+    msz = (C.c_int32 * max(2 * len(maps), 1))(*[v for m in maps for v in (int(m.shape[1]), int(m.shape[0]))])
+    a = make_args("gssdf_undistort_u8_args", n_frames=n, n_bytes=src.numel(), src=src, dst=dst, offsets=C.addressof(off),
+                  sizes=C.addressof(sz), map_ids=C.addressof(ids), n_maps=len(maps), maps=C.addressof(mp), map_sizes=C.addressof(msz))
+    check(lib().gssdf_undistort_u8(_lib.C.byref(a), _stream()))
+
+
 # ---- SDF branch -------------------------------------------------------------------------------
 def sdf_net(table_half, mlp, n_levels=16, n_features=2, log2_hashmap_size=19, base_resolution=32, per_level_scale=2.0,
             hidden_dim=64, n_hidden=3, origin=(0.0, 0.0, 0.0), inv_size=0.0, mlp_mode=0, mlp_packed=None):

@@ -1,5 +1,6 @@
 // gssdf::render_frames and gssdf::render_depth_normal_frames (shim/include/gssdf_frames.hpp) over the C ABI's gssdf_render_frames_u8 and
-// gssdf_render_depth_normal_u8, as gssdf_b200.views.render_frames and .render_depth_normal do it.
+// gssdf_render_depth_normal_u8, as gssdf_b200.views.render_frames and .render_depth_normal do it; gssdf::undistort_map and
+// gssdf::undistort over gssdf_undistort_map and gssdf_undistort_u8, as gssdf_b200.cameras does it.
 #include "gssdf_frames.hpp"
 
 #include <ATen/cuda/CUDAContext.h>
@@ -7,6 +8,7 @@
 
 #include <algorithm>
 #include <stdexcept>
+#include <vector>
 
 #include "../../include/gssdf_b200.h"
 
@@ -68,4 +70,46 @@ torch::Tensor gssdf::render_depth_normal_frames(const torch::Tensor &depth, cons
     a.render_alphas = al.data_ptr<float>(), a.normal = out.data_ptr<uint8_t>();
     check(gssdf_render_depth_normal_u8(&a, reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream())));
     return out;
+}
+
+torch::Tensor gssdf::undistort_map(const torch::Tensor &K, const torch::Tensor &D, const torch::Tensor &new_K, int64_t model, int64_t W,
+                                   int64_t H) {
+    for (const torch::Tensor *t : {&K, &D, &new_K})
+        TORCH_CHECK(!t->is_cuda() && t->scalar_type() == torch::kFloat, "K, D and new_K must be float32 CPU tensors");
+    TORCH_CHECK(K.numel() == 9 && new_K.numel() == 9 && D.numel() <= 5, "K and new_K must hold 9 values, D at most 5");
+    TORCH_CHECK(W >= 1 && H >= 1 && W <= INT32_MAX && H <= INT32_MAX, "bad map size ", W, " x ", H);
+    const torch::Tensor k = K.contiguous(), d = D.contiguous(), nk = new_K.contiguous();
+    gssdf_undistort_map_args a{};
+    a.model = (int32_t)model, a.W = (int32_t)W, a.H = (int32_t)H;
+    std::copy(k.data_ptr<float>(), k.data_ptr<float>() + 9, a.K);
+    std::copy(d.data_ptr<float>(), d.data_ptr<float>() + d.numel(), a.D);
+    std::copy(nk.data_ptr<float>(), nk.data_ptr<float>() + 9, a.new_K);
+    torch::Tensor map = torch::empty({H, W, 4}, torch::TensorOptions().dtype(torch::kShort).device(torch::kCUDA, c10::cuda::current_device()));
+    a.map = map.data_ptr<int16_t>();
+    check(gssdf_undistort_map(&a, reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream())));
+    return map;
+}
+
+torch::Tensor gssdf::undistort(const torch::Tensor &frames_u8, const torch::Tensor &map) {
+    TORCH_CHECK(frames_u8.is_cuda() && map.is_cuda() && frames_u8.device() == map.device(), "frames_u8 and map must be CUDA tensors on one device");
+    TORCH_CHECK(frames_u8.scalar_type() == torch::kByte && map.scalar_type() == torch::kShort, "frames_u8 must be uint8 and map int16");
+    TORCH_CHECK(map.dim() == 3 && map.size(2) == 4 && map.is_contiguous(), "map must be a contiguous int16 [H,W,4] of undistort_map");
+    const torch::Tensor f = (frames_u8.dim() == 3 ? frames_u8.unsqueeze(0) : frames_u8).contiguous();
+    TORCH_CHECK(f.dim() == 4 && f.size(1) == map.size(0) && f.size(2) == map.size(1) && f.size(3) == 3,
+                "frames_u8 must be [H,W,3] or [B,H,W,3] with the map's H and W");
+    const c10::cuda::CUDAGuard guard(f.device());
+    torch::Tensor out = torch::empty_like(f);
+    const int64_t B = f.size(0), frame = 3 * f.size(1) * f.size(2);
+    std::vector<int64_t> offsets(B);
+    std::vector<int32_t> sizes(2 * B), ids(B, 0);
+    for (int64_t b = 0; b < B; ++b) offsets[b] = b * frame, sizes[2 * b] = (int32_t)f.size(2), sizes[2 * b + 1] = (int32_t)f.size(1);
+    const int16_t *maps[1] = {map.data_ptr<int16_t>()};
+    const int32_t map_sizes[2] = {(int32_t)map.size(1), (int32_t)map.size(0)};
+    gssdf_undistort_u8_args a{};
+    a.n_frames = (int32_t)B, a.n_bytes = f.numel();
+    a.src = f.data_ptr<uint8_t>(), a.dst = out.data_ptr<uint8_t>();
+    a.offsets = offsets.data(), a.sizes = sizes.data(), a.map_ids = ids.data();
+    a.n_maps = 1, a.maps = maps, a.map_sizes = map_sizes;
+    check(gssdf_undistort_u8(&a, reinterpret_cast<gssdf_stream_t>(at::cuda::getCurrentCUDAStream().stream())));
+    return frames_u8.dim() == 3 ? out.squeeze(0) : out;
 }

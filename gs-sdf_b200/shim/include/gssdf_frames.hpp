@@ -17,4 +17,14 @@ std::vector<torch::Tensor> render_frames(const torch::Tensor &out_colors, const 
 // world->camera; Ks [C,3,3]; float32 CUDA tensors on one device ([H,W,*] and [4,4] / [3,3] are read as one view). No host sync.
 torch::Tensor render_depth_normal_frames(const torch::Tensor &depth, const torch::Tensor &render_alphas, const torch::Tensor &viewmats,
                                          const torch::Tensor &Ks);
+
+// sensor::Cameras' undistortion (DESIGN 7r, INTEGRATION 3o), in place of cv::initUndistortRectifyMap / cv::fisheye::initUndistortRectifyMap
+// (CV_16SC2) and cv::remap(INTER_LINEAR) in set_distortion / undistort; the node still takes new_K from cv::getOptimalNewCameraMatrix.
+// undistort_map: the map of one camera, int16 [H,W,4] on the current CUDA device (gssdf_undistort_map). K, new_K: 3x3 and D: at most 5
+// coefficients (k1 k2 p1 p2 k3 for model 0, k1..k4 for model 1), float32 CPU tensors (the cv::Mat values). The same map as
+// gssdf_b200.cameras.Undistortion.map.
+torch::Tensor undistort_map(const torch::Tensor &K, const torch::Tensor &D, const torch::Tensor &new_K, int64_t model, int64_t W, int64_t H);
+// undistort: uint8 [H,W,3] or [B,H,W,3] CUDA frames (RGB or BGR: each channel is remapped alone) through one map of their size on their
+// device, as a new tensor of the same shape (gssdf_undistort_u8); the same bytes as gssdf_b200.cameras.undistort_frames. No host sync.
+torch::Tensor undistort(const torch::Tensor &frames_u8, const torch::Tensor &map);
 }  // namespace gssdf

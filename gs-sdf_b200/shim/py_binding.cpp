@@ -73,6 +73,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("gssdf_psnr", &gssdf::psnr);
     m.def("gssdf_image_metrics", &gssdf::image_metrics, pybind11::arg("renders"), pybind11::arg("gts"), pybind11::arg("input_mode") = 2);
     m.def("gssdf_render_frames", &gssdf::render_frames, pybind11::arg("out_colors"), pybind11::arg("out_normals"));
+    m.def("gssdf_undistort_map", &gssdf::undistort_map, pybind11::arg("K"), pybind11::arg("D"), pybind11::arg("new_K"), pybind11::arg("model"),
+          pybind11::arg("W"), pybind11::arg("H"));
+    m.def("gssdf_undistort", &gssdf::undistort, pybind11::arg("frames_u8"), pybind11::arg("map"));
     m.def("gssdf_render_depth_normal_frames", &gssdf::render_depth_normal_frames, pybind11::arg("depth"), pybind11::arg("render_alphas"),
           pybind11::arg("viewmats"), pybind11::arg("Ks"));
     m.def("gssdf_eval_render", &gssdf::eval_render, pybind11::arg("renders"), pybind11::arg("gts"), pybind11::arg("names"),

@@ -1511,6 +1511,60 @@ typedef struct gssdf_frames_u8_expand_args {
 } gssdf_frames_u8_expand_args;
 int gssdf_frames_u8_expand(const gssdf_frames_u8_expand_args *a, gssdf_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * f-17  Undistortion of colour frames.  Replaces cv::initUndistortRectifyMap (model 0) / cv::fisheye::initUndistortRectifyMap
+ *     (model 1) with CV_16SC2 maps and cv::remap(INTER_LINEAR) inside sensor::Cameras (include/utils/sensor_utils/cameras.hpp:63-131),
+ *     which the reference runs on every raw, train and eval colour frame of a distorted camera (DESIGN 7r). The new camera matrix of
+ *     set_distortion (cv::getOptimalNewCameraMatrix) stays on the host (gssdf_b200.cameras). No allocation, no host sync, no
+ *     workspace; every argument is checked before the first launch.
+ * ------------------------------------------------------------------------------------------ */
+/* One camera's map, built once: for the output (undistorted) pixel (j, i), in fp64 with every product, sum and quotient rounded once
+   (no FMA contraction) and ir = inv(new_K) by the 3x3 cofactor formula of cv::invert(DECOMP_LU):
+     X = (i ir[1] + ir[2]) + j ir[0],  Y = (i ir[4] + ir[5]) + j ir[3],  Z = (i ir[7] + ir[8]) + j ir[6]
+     model 0:  x = X (1/Z), y = Y (1/Z), r2 = x x + y y, kr = 1 + ((k3 r2 + k2) r2 + k1) r2
+               u = fx (x kr + p1 (2x y) + p2 (r2 + 2 x x)) + cx,   v = fy (y kr + p1 (r2 + 2 y y) + p2 (2x y)) + cy
+     model 1:  x = X / Z, y = Y / Z, r = sqrt(x x + y y), t = atan(r), td = t (1 + k1 t^2 + k2 t^4 + k3 t^6 + k4 t^8) (left to right)
+               u = fx x s + cx, v = fy y s + cy with s = td / r (1 at r = 0)
+     iu = cvRound(u * 32), iv = cvRound(v * 32)   (ties to even; outside int32 or NaN -> INT_MIN)
+     map[i, j] = (saturate_s16(iu >> 5), saturate_s16(iv >> 5), (iv & 31) * 32 + (iu & 31), 0)
+   K, D, new_K are fp32 (D = k1 k2 p1 p2 k3 for model 0, k1 k2 k3 k4 for model 1). Equal to OpenCV's map wherever OpenCV's vectorised
+   and scalar code paths agree with each other: they can differ in the last bit where u * 32 is exactly a half-integer, and OpenCV
+   casts (wraps) instead of saturating iu >> 5 in the scalar tail of a row; both need source coordinates beyond +-32767 px or intrinsics
+   chosen to hit the 1/64 px grid. atan is the device's (2 ulp). GSSDF_EINVAL before any launch for W or H < 1, W H > 2^29, an unknown
+   model, a NULL or not 8-byte aligned map, or a non-finite K, D or new_K entry. */
+typedef struct gssdf_undistort_map_args {
+    int32_t model;                /* 0 radial-tangential, 1 equidistant (fisheye) */
+    int32_t W, H;                 /* frame size (distorted and undistorted) */
+    float K[9];                   /* the distorted camera, row-major */
+    float D[5];                   /* distortion coefficients; model 1 reads D[0..3] */
+    float new_K[9];               /* the undistorted pinhole camera, row-major */
+    int16_t *map;                 /* [H,W,4] device, overwritten */
+} gssdf_undistort_map_args;
+int gssdf_undistort_map(const gssdf_undistort_map_args *a, gssdf_stream_t stream);
+
+/* Remap a batch of packed interleaved 8-bit RGB frames (gstrain.FramesU8's layout: frame f is W_f H_f 3 bytes at byte offsets[f]) into
+   a second store of the same layout through the map of each frame's camera. Per output pixel p of frame f, with (sx, sy, frac) =
+   maps[map_ids[f]][p], a = frac & 31, b = (frac >> 5) & 31 and per channel
+     dst = (  (32-a)(32-b) src[sy][sx] + a(32-b) src[sy][sx+1] + (32-a)b src[sy+1][sx] + ab src[sy+1][sx+1] + 512 ) >> 10
+   where a tap outside the frame reads 0 (BORDER_CONSTANT 0: a pixel whose 2x2 block lies wholly outside is 0). This is cv::remap's
+   BilinearTab_i arithmetic, (acc + 2^14) >> 15 with weights 32x these. The map must have the frame's size. Bit-identical from run to
+   run and whatever the batch. Up to 32 frames per launch. GSSDF_EINVAL before any launch for n_frames < 0, n_maps < 1 (when
+   n_frames > 0), a NULL pointer, a frame or map size outside W, H >= 1, W H <= 2^29, a frame that does not fit n_bytes, a map id out
+   of range, a map whose size is not its frame's, a map not 8-byte aligned, or src and dst that overlap. n_frames == 0 is a no-op. */
+typedef struct gssdf_undistort_u8_args {
+    int32_t n_frames;
+    int64_t n_bytes;              /* bytes of src and of dst */
+    const uint8_t *src;           /* device */
+    uint8_t *dst;                 /* device, overwritten where frames lie */
+    const int64_t *offsets;       /* host [n_frames] byte offset of frame f in src and dst */
+    const int32_t *sizes;         /* host [n_frames,2] W_f, H_f */
+    const int32_t *map_ids;       /* host [n_frames] */
+    int32_t n_maps;
+    const int16_t *const *maps;   /* host [n_maps] device maps [H,W,4] of gssdf_undistort_map */
+    const int32_t *map_sizes;     /* host [n_maps,2] W, H */
+} gssdf_undistort_u8_args;
+int gssdf_undistort_u8(const gssdf_undistort_u8_args *a, gssdf_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
